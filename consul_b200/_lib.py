@@ -115,6 +115,9 @@ SIGNATURES = [
     ("gsim_user_event", _i32, [_P, _u32, C.c_char_p, _sz, C.c_char_p, _sz, _i32, C.POINTER(_u32)]),
     ("gsim_rumor_inject", _i32, [_P, _u32, _u32, C.POINTER(_i32)]),
     ("gsim_latency_set", _i32, [_P, _u32, C.POINTER(C.c_uint8)]),
+    ("gsim_impair_many", _i32, [_P, C.POINTER(_u32), _sz, _u32, _u32]),
+    ("gsim_impair_fraction", _i32, [_P, _u32, _u32, _u32, _u32, C.POINTER(_u32)]),
+    ("gsim_impair_get", _i32, [_P, _u32, C.POINTER(_u32), C.POINTER(_u32)]),
     ("gsim_graph_set", _i32, [_P, _u32, C.POINTER(_u32), C.POINTER(_u32)]),
     ("gsim_member_reconnect_timeout_set", _i32, [_P, _u32, _u64]),
     ("gsim_coordinate_get", _i32, [_P, _u32, C.POINTER(C.c_double)]),

@@ -290,6 +290,11 @@ struct gsim_pool {
   uint32_t retry_at = 0;     // do not look for quietness again before this tick
   // window launches, ticks run in windows, single-tick launches, horizon scans, ns of window kernels, ns of tick kernels
   uint64_t sched_counts[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  // degraded members (gsim_impair_*): the columns, allocated on first use, and how many members have a
+  // non-zero impairment.  d.imp_loss / d.imp_delay point at the columns only while that count is > 0.
+  uint32_t* imp_loss = nullptr;
+  uint8_t* imp_delay = nullptr;
+  uint32_t n_impaired = 0;
 };
 
 static void counts_invalidate(gsim_pool* p) {
@@ -1591,6 +1596,130 @@ extern "C" int gsim_member_watch(gsim_pool* p, uint32_t id, int on) {
   });
 }
 
+// ---- degraded members (DESIGN.md §3) -------------------------------------------------------
+// Loss in ppm -> the Philox threshold (the rule of packet_loss_ppm), and back: thr = floor(ppm 2^32 / 1e6)
+// is one-to-one because 2^32 / 1e6 > 1, so ppm = ceil(thr 1e6 / 2^32).
+static uint32_t ppm_to_thr(uint32_t ppm) {
+  return ppm >= 1000000u ? 0xFFFFFFFFu : (uint32_t)(((uint64_t)ppm << 32) / 1000000ull);
+}
+static uint32_t thr_to_ppm(uint32_t thr) { return (uint32_t)(((uint64_t)thr * 1000000ull + 0xFFFFFFFFull) >> 32); }
+
+// largest extra one-way latency of the datacenter matrix (0 without one)
+static uint32_t max_dc_extra(const GsGlobals& g) {
+  uint32_t m = 0;
+  for (uint32_t a = 0; a < g.n_dcs; ++a)
+    for (uint32_t b = 0; b < g.n_dcs; ++b) m = g.lat[a * GS_MAX_DCS + b] > m ? g.lat[a * GS_MAX_DCS + b] : m;
+  return m;
+}
+
+static bool impair_max_delay(gsim_pool* p, uint32_t* out) {
+  *out = 0;
+  if (!p->imp_delay || !p->g.n) return true;
+  std::vector<uint8_t> v(p->g.n);
+  if (!p->be->d2h(v.data(), p->imp_delay, v.size())) return false;
+  for (uint8_t x : v) *out = x > *out ? x : *out;
+  return true;
+}
+
+static bool impair_alloc(gsim_pool* p) {
+  if (p->imp_loss) return true;
+  const size_t cap = p->g.cap;
+  uint32_t* loss = nullptr;
+  uint8_t* delay = nullptr;
+  if (!alloc_col(p, &loss, cap) || !alloc_col(p, &delay, cap)) return false;
+  if (!p->be->fill32(loss, 0, cap) || !p->be->fill8(delay, 0, cap)) return false;
+  p->imp_loss = loss;
+  p->imp_delay = delay;
+  return true;
+}
+
+// The kernels see the columns only while somebody is impaired: with none, every path (fast paths, long
+// windows, closed form) is exactly the one of a pool that never was.
+static void impair_publish(gsim_pool* p) {
+  p->d.imp_loss = p->n_impaired ? p->imp_loss : nullptr;
+  p->d.imp_delay = p->n_impaired ? p->imp_delay : nullptr;
+  mark_dirty(p);
+}
+
+static bool impair_recount(gsim_pool* p) {
+  p->n_impaired = 0;
+  if (p->imp_loss && p->g.n) {
+    std::vector<uint32_t> loss(p->g.n);
+    std::vector<uint8_t> delay(p->g.n);
+    if (!p->be->d2h(loss.data(), p->imp_loss, loss.size() * 4) || !p->be->d2h(delay.data(), p->imp_delay, delay.size()))
+      return false;
+    for (uint32_t i = 0; i < p->g.n; ++i) p->n_impaired += (loss[i] | delay[i]) != 0u ? 1u : 0u;
+  }
+  impair_publish(p);
+  return true;
+}
+
+static int impair_check(gsim_pool* p, uint32_t loss_ppm, uint32_t delay_ticks) {
+  if (p->sharded) return fail(p, GSIM_ERR_STATE, "member impairment is not supported on sharded pools");
+  if (loss_ppm > 1000000u) return fail(p, GSIM_ERR_INVALID, "loss_ppm must be <= 1000000");
+  // a packet to the member arrives 1 + extra + delay ticks after it was sent: that slot must not wrap the ring
+  if ((uint64_t)max_dc_extra(p->g) + delay_ticks + 2u > (uint64_t)p->g.ring_mask + 1u)
+    return fail(p, GSIM_ERR_INVALID, "latency plus receive delay must stay below mailbox_depth - 1 extra ticks");
+  return GSIM_OK;
+}
+
+extern "C" int gsim_impair_many(gsim_pool* p, const uint32_t* ids, size_t n, uint32_t loss_ppm, uint32_t delay_ticks) {
+  if (!p || (!ids && n)) return GSIM_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(p->mu);
+  int rc = impair_check(p, loss_ppm, delay_ticks);
+  if (rc) return rc;
+  for (size_t x = 0; x < n; ++x)
+    if (ids[x] >= p->g.n) return fail(p, GSIM_ERR_NOT_FOUND, "unknown member");
+  const uint32_t thr = ppm_to_thr(loss_ppm);
+  const bool now_impaired = thr != 0u || delay_ticks != 0u;
+  if (!p->imp_loss && !now_impaired) return GSIM_OK;  // clearing on a pool that never was impaired
+  if (!impair_alloc(p)) return fail(p, GSIM_ERR_NOMEM, "impairment columns");
+  for (size_t x = 0; x < n; ++x) {
+    uint32_t old_loss;
+    uint8_t old_delay;
+    if (!peek(p, p->imp_loss, ids[x], &old_loss) || !peek(p, p->imp_delay, ids[x], &old_delay))
+      return fail(p, GSIM_ERR_CUDA, "peek");
+    const bool was = old_loss != 0u || old_delay != 0u;
+    if (!poke(p, p->imp_loss, ids[x], thr) || !poke(p, p->imp_delay, ids[x], (uint8_t)delay_ticks))
+      return fail(p, GSIM_ERR_CUDA, "poke");
+    p->n_impaired = p->n_impaired - (was ? 1u : 0u) + (now_impaired ? 1u : 0u);
+  }
+  impair_publish(p);
+  return GSIM_OK;
+}
+
+extern "C" int gsim_impair_fraction(gsim_pool* p, uint32_t member_ppm, uint32_t salt, uint32_t loss_ppm,
+                                    uint32_t delay_ticks, uint32_t* n_impaired) {
+  if (!p || member_ppm > 1000000u) return GSIM_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(p->mu);
+  int rc = impair_check(p, loss_ppm, delay_ticks);
+  if (rc) return rc;
+  if (!impair_alloc(p)) return fail(p, GSIM_ERR_NOMEM, "impairment columns");
+  if (!upload_globals(p)) return fail(p, GSIM_ERR_CUDA, "upload");
+  const uint32_t thr = ppm_to_thr(loss_ppm);
+  uint32_t counts[2] = {0, 0};
+  if (!p->be->impair_fraction(p->d, p->g_dev, p->g, p->imp_loss, p->imp_delay, ppm_to_thr(member_ppm), salt, thr,
+                              delay_ticks, counts))
+    return fail(p, GSIM_ERR_CUDA, "impair_fraction");
+  p->n_impaired = p->n_impaired - counts[1] + (thr != 0u || delay_ticks != 0u ? counts[0] : 0u);
+  if (n_impaired) *n_impaired = counts[0];
+  impair_publish(p);
+  return GSIM_OK;
+}
+
+extern "C" int gsim_impair_get(gsim_pool* p, uint32_t id, uint32_t* loss_ppm, uint32_t* delay_ticks) {
+  if (!p) return GSIM_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(p->mu);
+  if (id >= p->g.n) return fail(p, GSIM_ERR_NOT_FOUND, "unknown member");
+  uint32_t thr = 0;
+  uint8_t delay = 0;
+  if (p->imp_loss && (!peek(p, p->imp_loss, id, &thr) || !peek(p, p->imp_delay, id, &delay)))
+    return fail(p, GSIM_ERR_CUDA, "peek");
+  if (loss_ppm) *loss_ppm = thr_to_ppm(thr);
+  if (delay_ticks) *delay_ticks = delay;
+  return GSIM_OK;
+}
+
 // WAN latency pools (BASELINE config 5, SURVEY 8d C5): n_dcs synthetic datacenters, member i
 // lives in datacenter (i / 128) % n_dcs; a packet from datacenter a to b takes lat[a*n_dcs+b]
 // ticks (>= 1; 1 is the latency every packet has on a pool without a matrix).
@@ -1599,9 +1728,13 @@ extern "C" int gsim_latency_set(gsim_pool* p, uint32_t n_dcs, const uint8_t* lat
   std::lock_guard<std::mutex> lk(p->mu);
   return controller_call(p, nullptr, 0, [&]() -> int {
   GsGlobals& g = p->g;
+  uint32_t max_delay = 0;
+  if (p->n_impaired && !impair_max_delay(p, &max_delay)) return fail(p, GSIM_ERR_CUDA, "d2h");
   for (uint32_t x = 0; x < n_dcs * n_dcs; ++x)
     if (lat_ticks[x] < 1u || lat_ticks[x] > g.ring_mask)
       return fail(p, GSIM_ERR_INVALID, "latency must be in [1, mailbox_depth - 1] ticks");
+    else if (lat_ticks[x] + max_delay > g.ring_mask)
+      return fail(p, GSIM_ERR_INVALID, "latency plus the largest receive delay must stay below mailbox_depth");
   memset(g.lat, 0, sizeof(g.lat));
   for (uint32_t a = 0; a < n_dcs; ++a)
     for (uint32_t b = 0; b < n_dcs; ++b) g.lat[a * GS_MAX_DCS + b] = (uint8_t)(lat_ticks[a * n_dcs + b] - 1u);
@@ -1753,7 +1886,7 @@ static int try_quiet(gsim_pool* p) {
     for (uint32_t a = 0; a < g.n_dcs && links_ok; ++a)
       for (uint32_t b = 0; b < g.n_dcs; ++b)
         if ((uint32_t)g.lat[a * GS_MAX_DCS + b] + g.lat[b * GS_MAX_DCS + a] > g.T) links_ok = false;
-    if (hz == GS_NEVER && g.loss_thr == 0u && links_ok) {
+    if (hz == GS_NEVER && g.loss_thr == 0u && p->n_impaired == 0u && links_ok) {
       counts_invalidate(p);  // (ticks have run since the last count)
       int rc = collective_recount(p);
       if (rc) return rc;
@@ -2296,7 +2429,7 @@ struct SnapCol {
   uint32_t planes;   // equally sized, each a multiple of 4 bytes
   bool may_fill;     // planes may be stored as a repeated word
 };
-static std::vector<SnapCol> snap_cols(gsim_pool* p) {
+static std::vector<SnapCol> snap_cols(gsim_pool* p, bool with_impairment) {
   const GsDev& d = p->d;
   const size_t cap = p->g.cap;
   std::vector<SnapCol> v;
@@ -2319,6 +2452,10 @@ static std::vector<SnapCol> snap_cols(gsim_pool* p) {
   if (d.ppreq) {
     add(d.ppreq, cap * 4 * 2 * GS_PPK, 2 * GS_PPK);
     add(d.pp_clk, cap * 4 * 4, 4);
+  }
+  if (with_impairment) {
+    add(p->imp_loss, cap * 4);
+    add(p->imp_delay, cap);
   }
   add(d.stats, GSIM_STAT_COUNT * 8, 1, false); add(d.heard_cnt, 32 * 4, 1, false); add(d.conv_tick, 32 * 4, 1, false);
   add(d.crashed_alive, 4, 1, false); add(d.crashed_dead_tick, 4, 1, false);
@@ -2344,6 +2481,7 @@ static uint32_t snap_layout(const gsim_pool* p) {
   if (p->d.coord) m |= 1u;
   if (p->d.ppreq) m |= 2u;
   if (p->d.kst) m |= 4u;
+  if (p->imp_loss) m |= 8u;  // impairment columns (restore allocates them when the pool has none)
   if (p->sharded) m |= 16u;
   return m;
 }
@@ -2364,7 +2502,7 @@ static uint64_t snap_graph_hash(const gsim_pool* p) {
 static size_t snap_size(gsim_pool* p) {
   size_t s = sizeof(SnapHeader) + p->sched.size() * sizeof(Sched);
   for (uint32_t r = 0; r < GS_MAX_RUMORS; ++r) s += 12 + p->rh[r].name.size() + p->rh[r].payload.size();
-  for (const SnapCol& c : snap_cols(p)) s += c.bytes + 4u * c.planes;  // upper bound: every plane raw
+  for (const SnapCol& c : snap_cols(p, p->imp_loss != nullptr)) s += c.bytes + 4u * c.planes;  // upper bound: every plane raw
   return s;
 }
 
@@ -2411,7 +2549,7 @@ extern "C" int gsim_snapshot(gsim_pool* p, void* out, size_t cap_bytes, size_t* 
     memcpy(w, p->rh[r].payload.data(), hdr[1]);
     w += hdr[1];
   }
-  for (const SnapCol& c : snap_cols(p)) {
+  for (const SnapCol& c : snap_cols(p, p->imp_loss != nullptr)) {
     const size_t pb = c.bytes / c.planes;
     for (uint32_t q = 0; q < c.planes; ++q) {
       uint8_t* raw = w + 4;
@@ -2441,7 +2579,7 @@ extern "C" int gsim_restore(gsim_pool* p, const void* blob, size_t n_bytes) {
   // geometry and peer graph must be this pool's before a single plane is copied.
   if (h.cap != p->g.cap || h.g.cap != p->g.cap || h.g.n > p->cfg.capacity || h.g.n > p->g.cap ||
       h.g.ring_mask != p->g.ring_mask || (h.g.pp_interval != 0u) != (p->g.pp_interval != 0u) ||
-      h.layout != snap_layout(p) || h.g.world != p->g.world || h.g.key_stride != p->g.key_stride ||
+      (h.layout & ~8u) != (snap_layout(p) & ~8u) || h.g.world != p->g.world || h.g.key_stride != p->g.key_stride ||
       h.g.rows_per_rank != p->g.rows_per_rank || h.g.phase_group != p->g.phase_group ||
       h.g.graph_n != p->g.graph_n || h.graph_hash != snap_graph_hash(p) || h.n_established > h.g.n)
     return fail(p, GSIM_ERR_INVALID, "snapshot does not match this pool (capacity, column set, sharding or peer graph)");
@@ -2461,7 +2599,9 @@ extern "C" int gsim_restore(gsim_pool* p, const void* blob, size_t n_bytes) {
     r += hdr[1];
     p->rh[x].coalesce = (int)hdr[2];
   }
-  for (const SnapCol& c : snap_cols(p)) {
+  const bool blob_impaired = (h.layout & 8u) != 0u;
+  if (blob_impaired && !impair_alloc(p)) return fail(p, GSIM_ERR_NOMEM, "impairment columns");
+  for (const SnapCol& c : snap_cols(p, blob_impaired)) {
     if (c.may_fill) {  // plane by plane: a device fill or a copy
       const size_t pb = c.bytes / c.planes;
       for (uint32_t q = 0; q < c.planes; ++q) {
@@ -2500,6 +2640,10 @@ extern "C" int gsim_restore(gsim_pool* p, const void* blob, size_t n_bytes) {
     }
     r += c.bytes;
   }
+  // a blob without impairment columns restores a pool nobody in it is impaired
+  if (!blob_impaired && p->imp_loss &&
+      (!p->be->fill32(p->imp_loss, 0, p->g.cap) || !p->be->fill8(p->imp_delay, 0, p->g.cap)))
+    return fail(p, GSIM_ERR_CUDA, "fill");
   if (!p->be->sync()) return fail(p, GSIM_ERR_CUDA, "sync");  // every plane has left the caller's blob
   {
     // topology fields stay the live pool's (they were checked equal above, except the rank, which is
@@ -2516,6 +2660,7 @@ extern "C" int gsim_restore(gsim_pool* p, const void* blob, size_t n_bytes) {
   p->n_established = h.n_established;
   p->g_dirty = true;
   counts_invalidate(p);
+  if (!impair_recount(p)) return fail(p, GSIM_ERR_CUDA, "d2h");
   if (!poke(p, p->d.tick_base, 0, p->now) || !reset_tick_flags(p) || !reset_qstate(p)) return fail(p, GSIM_ERR_CUDA, "poke");
   uint32_t zero2[2] = {0, 0};
   if (!p->be->h2d(p->d.evlog_cursor, zero2, 8)) return fail(p, GSIM_ERR_CUDA, "h2d");

@@ -8,6 +8,8 @@
 #include <stdint.h>
 #include <stdlib.h>
 
+#include <vector>
+
 #include "gs_core.h"
 
 struct GsRecount {
@@ -75,6 +77,27 @@ class GsBackend {
   virtual bool xbar_host(const GsXbar&) { return false; }  // arrive, wait for every rank, sync
   virtual bool crash_fraction(const GsDev& d, const GsGlobals* g_dev, const GsGlobals& g,
                               uint32_t thr, uint32_t salt, uint32_t now, uint32_t* n_crashed) = 0;
+  // gs_impair_row over every member, writing the impairment columns (allocated by the caller, who
+  // may not have published them in `d` yet); counts[0] = members selected, counts[1] = how many of
+  // them were impaired before.  Defined here through the copy primitives every backend has, which is
+  // what the host emulation runs; the CUDA backend replaces it with gs_impair_kernel.
+  virtual bool impair_fraction(const GsDev& d, const GsGlobals* /*g_dev*/, const GsGlobals& g, uint32_t* loss_col,
+                               uint8_t* delay_col, uint32_t thr, uint32_t salt, uint32_t loss, uint32_t delay,
+                               uint32_t counts[2]) {
+    counts[0] = counts[1] = 0u;
+    if (!g.n) return true;
+    std::vector<uint32_t> key(g.n), lc(g.n);
+    std::vector<uint8_t> dc(g.n);
+    if (!d2h(key.data(), d.key[0], (size_t)g.n * 4) || !d2h(lc.data(), loss_col, (size_t)g.n * 4) ||
+        !d2h(dc.data(), delay_col, g.n))
+      return false;
+    for (uint32_t i = 0; i < g.n; ++i) {
+      const uint32_t r = gs_impair_row(key[i], lc.data(), dc.data(), g.seed_lo, g.seed_hi, i, thr, salt, loss, delay);
+      counts[0] += r & 1u;
+      counts[1] += (r >> 1) & 1u;
+    }
+    return h2d(loss_col, lc.data(), (size_t)g.n * 4) && h2d(delay_col, dc.data(), g.n);
+  }
   // counts over members [first, first + count) (a rank of a sharded pool counts its own rows)
   virtual bool recount(const GsDev& d, const GsGlobals* g_dev, const GsGlobals& g, uint32_t now, uint32_t first,
                        uint32_t count, GsRecount* out) = 0;

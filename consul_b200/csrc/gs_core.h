@@ -58,7 +58,9 @@ enum {
   GS_PUR_RELAY = 4,
   GS_PUR_LOSS = 5,
   GS_PUR_CRASH = 6,
-  GS_PUR_PUSHPULL = 7
+  GS_PUR_PUSHPULL = 7,
+  // 8 = GS_PUR_COORD (gs_coord.h)
+  GS_PUR_IMPAIR = 9
 };
 // Loss "kind" (folded into the counter) — one draw per simulated UDP packet.
 enum {
@@ -280,6 +282,20 @@ GS_HD uint32_t gs_pristine_probes(uint32_t n, uint32_t bits, const GsU4& rk, uin
   return gs_pristine_probes_k(n, bits, rk, self, cursor, (w1 - due + P - 1u) / P, special, n_special);
 }
 
+// gsim_impair_fraction for member i whose key word (either buffer: truth is in both) is key: a member that
+// runs and whose Philox draw (its own purpose word, so the selection is independent of gs_crash_row's for the
+// same salt) is below thr gets the impairment (loss, delay).  Returns bit 0 = selected, bit 1 = it was
+// impaired before.
+GS_HD uint32_t gs_impair_row(uint32_t key, uint32_t* loss_col, uint8_t* delay_col, uint32_t seed_lo, uint32_t seed_hi,
+                             uint32_t i, uint32_t thr, uint32_t salt, uint32_t loss, uint32_t delay) {
+  if ((key & 3u) != GS_TRUTH_UP) return 0u;
+  if (gs_philox(seed_lo, seed_hi, i, salt, GS_PUR_IMPAIR, 0u).x >= thr) return 0u;
+  const bool was = loss_col[i] != 0u || delay_col[i] != 0u;
+  loss_col[i] = loss;
+  delay_col[i] = (uint8_t)delay;
+  return was ? 3u : 1u;
+}
+
 // Retransmit counter of rumor r at member i.  Two rumors share one 16-bit element so that the
 // narrowest column has 2-byte elements: a sharded pool maps every (column, rank) slice with the
 // 2 MB granularity of the virtual-memory API, which then allows 1 Mi members per GPU (1-byte
@@ -406,6 +422,11 @@ struct GsDev {
   const uint32_t* col_idx;  // [row_ptr[graph_n]]
   uint32_t* ppreq;   // [2][GS_PPK][cap] requester ids, kept as the GS_PPK smallest (atomicMin chain)
   uint32_t* pp_clk;  // [2][2][cap] max of the senders' {member, event} Lamport clocks (atomicMax)
+  // degraded members (gsim_impair_*): per-member UDP loss threshold and receive delay in ticks.  Both
+  // null unless at least one member is impaired right now, which is also what turns the probe fast
+  // paths off (the host keeps the columns and the count; a pool that was never impaired has neither).
+  const uint32_t* imp_loss;  // [cap] packet to or from the member lost iff a Philox word < imp_loss
+  const uint8_t* imp_delay;  // [cap] extra ticks before the member handles what it receives
   // pool-wide device words
   unsigned long long* stats;  // [GSIM_STAT_COUNT]
   uint32_t* heard_cnt;        // [GS_MAX_RUMORS]

@@ -163,11 +163,23 @@ __device__ __forceinline__ void gs_q_publish(const GsDev& d, const GsGlobals& g,
 // registers (80 -> 3 resident CTAs per SM); as a call it costs the members that take it ~30
 // instructions on top of several hundred, and the loops around it fit 64 registers (4 CTAs per SM:
 // a quarter more warps to hide the L2 round trips, and at 1 M members two tiles per warp, not three).
+// Pools with degraded members step through an instantiation of their own, so the one every other pool runs
+// carries none of the impairment terms.
+template <bool COORDS>
+__device__ __noinline__ void gs_row_step_impaired_call(const GsDev* dp, const GsGlobals* gp, uint32_t i, uint32_t t,
+                                                       uint32_t inb, uint32_t* s_stat, uint32_t* s_heard, uint32_t* s_q) {
+  DevSinkT<COORDS> sink{s_stat, s_heard, s_q};
+  gs_row_step_body<true>(*dp, *gp, i, t, t % gp->GI, inb, sink);
+}
 template <bool COORDS>
 __device__ __noinline__ void gs_row_step_call(const GsDev* dp, const GsGlobals* gp, uint32_t i, uint32_t t,
                                               uint32_t inb, uint32_t* s_stat, uint32_t* s_heard, uint32_t* s_q) {
+  if (dp->imp_loss != nullptr) {
+    gs_row_step_impaired_call<COORDS>(dp, gp, i, t, inb, s_stat, s_heard, s_q);
+    return;
+  }
   DevSinkT<COORDS> sink{s_stat, s_heard, s_q};
-  gs_row_step(*dp, *gp, i, t, t % gp->GI, inb, sink);
+  gs_row_step_body<false>(*dp, *gp, i, t, t % gp->GI, inb, sink);
 }
 
 // Persistent, warp-centric tick.  Every warp owns a CONTIGUOUS chunk of tiles (128 members
@@ -431,7 +443,8 @@ __device__ __noinline__ void gs_window_generic(const GsDev* dp, const GsGlobals*
   const GsHot h = gs_hot(g);
   const uint32_t P = h.P, T = h.T, lane = threadIdx.x & 31u;
   const uint32_t tf0[4] = {tf00, tf01, tf02, tf03}, tx0[4] = {tx00, tx01, tx02, tx03};
-  const bool fast_ok = h.loss_thr == 0u && h.graph_n == 0u && d.coord == nullptr && h.pp_interval == 0u;
+  const bool fast_ok =
+      h.loss_thr == 0u && h.graph_n == 0u && d.coord == nullptr && d.imp_loss == nullptr && h.pp_interval == 0u;
   DevSinkT<COORDS> sink{s_stat, s_heard, s_q};
   uint32_t n_probe = 0, n_ack = 0;
   bool did_work = false;
@@ -567,7 +580,8 @@ __global__ void __launch_bounds__(GS_BLOCK, PRISTINE ? GS_WIN_BLOCKS_CLOSED : GS
   const uint32_t shift = g.phase_shift + 2u, t0_mod = t0 % P, rot_p = g.rot_p;
   const uint32_t win_q = (w1 - t0) / P, win_r = (w1 - t0) - win_q * P;
   // the batch is taken through the probe fast path together if the pool allows the fast path at all
-  const bool fast_ok = h.loss_thr == 0u && h.graph_n == 0u && d.coord == nullptr && h.pp_interval == 0u;
+  const bool fast_ok =
+      h.loss_thr == 0u && h.graph_n == 0u && d.coord == nullptr && d.imp_loss == nullptr && h.pp_interval == 0u;
   DevSinkT<COORDS> sink{s_stat, s_heard, s_q};
   bool did_work = false;
   uint32_t n_probe = 0, n_ack = 0;
@@ -753,7 +767,7 @@ __global__ void __launch_bounds__(GS_BLOCK, PRISTINE ? GS_WIN_BLOCKS_CLOSED : GS
             if (!go[u]) continue;
             const uint32_t i = (gb + u) * 32u + lane;
             if (gs_key_truth(kc[u]) != GS_TRUTH_UP || gs_key_rank(kc[u]) != GS_RANK_ALIVE || gs_key_pending(kc[u]) ||
-                gs_extra(h, i, c[u]) + gs_extra(h, c[u], i) > T) {
+                gs_extra(h, nullptr, i, c[u]) + gs_extra(h, nullptr, c[u], i) > T) {
               live[u] = false;  // anything but a prompt ack: the generic step decides
               continue;
             }
@@ -888,6 +902,19 @@ __global__ void __launch_bounds__(GS_BLOCK)
   if (i < gp->n) c = gs_crash_row(d, *gp, i, thr, salt);
   unsigned b = __ballot_sync(0xFFFFFFFFu, c);
   if ((threadIdx.x & 31u) == 0u && b) atomicAdd(n_crashed, (uint32_t)__popc(b));
+}
+
+__global__ void __launch_bounds__(GS_BLOCK)
+    gs_impair_kernel(GsDev d, const GsGlobals* __restrict__ gp, uint32_t* loss_col, uint8_t* delay_col, uint32_t thr,
+                     uint32_t salt, uint32_t loss, uint32_t delay, uint32_t* counts) {
+  const uint32_t i = blockIdx.x * GS_BLOCK + threadIdx.x;
+  uint32_t r = 0u;
+  if (i < gp->n) r = gs_impair_row(d.key[0][i], loss_col, delay_col, gp->seed_lo, gp->seed_hi, i, thr, salt, loss, delay);
+  const unsigned sel = __ballot_sync(0xFFFFFFFFu, r & 1u), was = __ballot_sync(0xFFFFFFFFu, r & 2u);
+  if ((threadIdx.x & 31u) == 0u && sel) {
+    atomicAdd(&counts[0], (uint32_t)__popc(sel));
+    if (was) atomicAdd(&counts[1], (uint32_t)__popc(was));
+  }
 }
 
 __global__ void __launch_bounds__(GS_BLOCK)
@@ -1279,6 +1306,19 @@ class CudaBackend : public GsBackend {
       ++launches_;
     }
     return ok(cudaGetLastError(), "crash launch") && d2h(n_crashed, cnt, 4);
+  }
+  bool impair_fraction(const GsDev& d, const GsGlobals* g_dev, const GsGlobals& g, uint32_t* loss_col,
+                       uint8_t* delay_col, uint32_t thr, uint32_t salt, uint32_t loss, uint32_t delay,
+                       uint32_t counts[2]) override {
+    cudaSetDevice(dev_);
+    uint32_t* cnt = reinterpret_cast<uint32_t*>(scratch_);
+    if (!ok(cudaMemsetAsync(cnt, 0, 8, stream_), "memset")) return false;
+    if (g.n) {
+      gs_impair_kernel<<<(g.n + GS_BLOCK - 1) / GS_BLOCK, GS_BLOCK, 0, stream_>>>(d, g_dev, loss_col, delay_col, thr,
+                                                                                  salt, loss, delay, cnt);
+      ++launches_;
+    }
+    return ok(cudaGetLastError(), "impair launch") && d2h(counts, cnt, 8);
   }
   bool reap_rows(const GsDev& d, const GsGlobals* g_dev, const GsGlobals& g, uint32_t now,
                  uint32_t reconnect_ticks, uint32_t tombstone_ticks, bool log_events,

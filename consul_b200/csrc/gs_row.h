@@ -196,28 +196,39 @@ GS_DEV GsHot gs_hot(const GsGlobals& g) {
   return h;
 }
 
+// `delay` = the receive-delay column of a pool with impaired members (GsDev::imp_delay), else null:
+// a degraded receiver handles everything delay[dst] ticks late.  The probe fast paths pass null,
+// they only run while nobody is impaired.
 template <class G>
-GS_DEV uint32_t gs_extra(const G& g, uint32_t src, uint32_t dst) {
-  if (g.n_dcs == 0u) return 0u;
-  return g.lat[((src / GS_TILE) % g.n_dcs) * GS_MAX_DCS + (dst / GS_TILE) % g.n_dcs];
+GS_DEV uint32_t gs_extra(const G& g, const uint8_t* delay, uint32_t src, uint32_t dst) {
+  uint32_t e = g.n_dcs == 0u ? 0u : g.lat[((src / GS_TILE) % g.n_dcs) * GS_MAX_DCS + (dst / GS_TILE) % g.n_dcs];
+  if (delay != nullptr) e += delay[dst];
+  return e;
+}
+
+// The loss rule of one simulated UDP packet from src to dst, on Philox block r of its counter: the
+// pool-wide draw (r.x), then the sender's and the receiver's own loss (r.y, r.z; `loss` =
+// GsDev::imp_loss, null while nobody is impaired).
+GS_DEV bool gs_loss_rule(const GsGlobals& g, const uint32_t* loss, const GsU4& r, uint32_t src, uint32_t dst) {
+  return r.x < g.loss_thr || (loss != nullptr && (r.y < loss[src] || r.z < loss[dst]));
 }
 
 // Same draw as gs_lost without touching the counters: re-evaluates, at the ProbeTimeout stage,
 // whether the direct ping/ack of the probe started at t0 were lost (late acks, latency pools).
-GS_DEV bool gs_lost_quiet(const GsGlobals& g, uint32_t src, uint32_t dst, uint32_t t, uint32_t kind,
-                          uint32_t idx) {
-  if (g.loss_thr == 0u) return false;
+GS_DEV bool gs_lost_quiet(const GsGlobals& g, const uint32_t* loss, uint32_t src, uint32_t dst, uint32_t t,
+                          uint32_t kind, uint32_t idx) {
+  if (g.loss_thr == 0u && loss == nullptr) return false;
   GsU4 r = gs_philox(g.seed_lo, g.seed_hi, src, dst, t, GS_PUR_LOSS | (kind << 8) | (idx << 16));
-  return r.x < g.loss_thr;
+  return gs_loss_rule(g, loss, r, src, dst);
 }
 
-// One simulated UDP packet is lost iff its Philox draw is below the threshold.
+// One simulated UDP packet is lost iff its Philox draw says so (gs_loss_rule); counted once.
 template <class Sink>
-GS_DEV bool gs_lost(const GsGlobals& g, Sink& sink, uint32_t src, uint32_t dst, uint32_t t,
+GS_DEV bool gs_lost(const GsGlobals& g, const uint32_t* loss, Sink& sink, uint32_t src, uint32_t dst, uint32_t t,
                     uint32_t kind, uint32_t idx) {
-  if (g.loss_thr == 0u) return false;
+  if (g.loss_thr == 0u && loss == nullptr) return false;
   GsU4 r = gs_philox(g.seed_lo, g.seed_hi, src, dst, t, GS_PUR_LOSS | (kind << 8) | (idx << 16));
-  bool lost = r.x < g.loss_thr;
+  bool lost = gs_loss_rule(g, loss, r, src, dst);
   if (lost) sink.stat(GS_ST_PACKETS_LOST, 1);
   return lost;
 }
@@ -281,7 +292,8 @@ __device__ __noinline__
 #else
 inline
 #endif
-void gs_coord_on_ack(double* coord, uint32_t* ctag, double* adj, uint32_t* adj_idx, const GsGlobals& g, uint32_t i,
+void gs_coord_on_ack(double* coord, uint32_t* ctag, double* adj, uint32_t* adj_idx, const uint8_t* imp_delay,
+                     const GsGlobals& g, uint32_t i,
                      uint32_t j, uint32_t t) {  // (column pointers by value: taking the address of the
                                                  // kernel's GsDev parameter would copy it to the stack)
   const size_t cap = g.cap;
@@ -290,7 +302,8 @@ void gs_coord_on_ack(double* coord, uint32_t* ctag, double* adj, uint32_t* adj_i
   GsCoord c, other;
   gs_coord_load(coord, cap, mine, i, c);
   gs_coord_load(coord, cap, gs_coord_slot_for_reader(ctag, cap, j, t), j, other);
-  const double rtt = g.coord_base_rtt_s + (double)(gs_extra(g, i, j) + gs_extra(g, j, i)) * g.tick_seconds;
+  const double rtt =
+      g.coord_base_rtt_s + (double)(gs_extra(g, imp_delay, i, j) + gs_extra(g, imp_delay, j, i)) * g.tick_seconds;
   uint32_t idx = adj_idx[i];
   gs_coord_client_update(c, other, rtt, adj + i, cap, &idx, g.seed_lo, g.seed_hi, i, t);
   adj_idx[i] = idx;
@@ -419,9 +432,14 @@ GS_DEV bool gs_tile_probe_gate(const GsGlobals& g, uint32_t tile, uint32_t pslot
 
 // The tick of member i, called only for rows that have mail (inb = inbox[t&1][i] != 0,
 // which includes the self-posted wake bit) or a probe action due (due[i] == t).
-template <class Sink>
-GS_DEV void gs_row_step(const GsDev& d, const GsGlobals& g, uint32_t i, uint32_t t, uint32_t gslot,
-                        uint32_t inb, Sink& sink) {
+// IMPAIRED: the pool has degraded members (GsDev::imp_loss / imp_delay are set).  The other
+// instantiation folds every impairment term away, so a pool without any runs the code it would
+// run without the feature.
+template <bool IMPAIRED, class Sink>
+GS_DEV void gs_row_step_body(const GsDev& d, const GsGlobals& g, uint32_t i, uint32_t t, uint32_t gslot,
+                             uint32_t inb, Sink& sink) {
+  const uint32_t* const imp_loss = IMPAIRED ? d.imp_loss : nullptr;
+  const uint8_t* const imp_delay = IMPAIRED ? d.imp_delay : nullptr;
   const uint32_t cur = t & 1u, nxt = cur ^ 1u;                            // key / acc buffers
   const uint32_t icur = t & g.ring_mask, inxt = (t + 1u) & g.ring_mask;  // mailbox ring slots
   const uint32_t k0 = d.key[cur][i];
@@ -623,25 +641,25 @@ GS_DEV void gs_row_step(const GsDev& d, const GsGlobals& g, uint32_t i, uint32_t
         const uint32_t r = relays[q];
         const bool r_up = gs_key_truth(gs_peer_key(d, cur, r, false)) == GS_TRUTH_UP;
         sink.stat(GS_ST_INDIRECT_PINGS, 1);
-        if (!(r_up && !gs_lost(g, sink, i, r, t, GS_LK_INDREQ, q))) continue;  // no nack either
-        const uint32_t via = gs_extra(g, i, r) + gs_extra(g, r, i);
-        const uint32_t rtt_rj = gs_extra(g, r, j) + gs_extra(g, j, r);
+        if (!(r_up && !gs_lost(g, imp_loss, sink, i, r, t, GS_LK_INDREQ, q))) continue;  // no nack either
+        const uint32_t via = gs_extra(g, imp_delay, i, r) + gs_extra(g, imp_delay, r, i);
+        const uint32_t rtt_rj = gs_extra(g, imp_delay, r, j) + gs_extra(g, imp_delay, j, r);
         // the relay waits ProbeTimeout for the target's ack, then answers with a nack
-        bool relay_acked = j_up && !gs_lost(g, sink, r, j, t, GS_LK_INDPING, q) &&
-                           !gs_lost(g, sink, j, r, t, GS_LK_INDACK, q) && rtt_rj <= g.T;
+        bool relay_acked = j_up && !gs_lost(g, imp_loss, sink, r, j, t, GS_LK_INDPING, q) &&
+                           !gs_lost(g, imp_loss, sink, j, r, t, GS_LK_INDACK, q) && rtt_rj <= g.T;
         if (relay_acked) {
-          if (!gs_lost(g, sink, r, i, t, GS_LK_INDFWD, q) && via + rtt_rj <= budget) success = true;
-        } else if (!gs_lost(g, sink, r, i, t, GS_LK_NACK, q) && via <= budget) {
+          if (!gs_lost(g, imp_loss, sink, r, i, t, GS_LK_INDFWD, q) && via + rtt_rj <= budget) success = true;
+        } else if (!gs_lost(g, imp_loss, sink, r, i, t, GS_LK_NACK, q) && via <= budget) {
           ++nacks;
           sink.stat(GS_ST_NACKS, 1);
         }
       }
       const uint32_t t0 = t - g.T;
-      const uint32_t rtt_ij = gs_extra(g, i, j) + gs_extra(g, j, i);
+      const uint32_t rtt_ij = gs_extra(g, imp_delay, i, j) + gs_extra(g, imp_delay, j, i);
       if (!g.disable_tcp && j_up && rtt_ij <= budget) success = true;  // TCP fallback ping is reliable
       // a direct ack that was merely slower than ProbeTimeout still counts until the deadline
-      if (g.n_dcs != 0u && j_up && rtt_ij > g.T && rtt_ij <= budget + g.T &&
-          !gs_lost_quiet(g, i, j, t0, GS_LK_PING, 0) && !gs_lost_quiet(g, j, i, t0, GS_LK_ACK, 0))
+      if ((g.n_dcs != 0u || imp_delay != nullptr) && j_up && rtt_ij > g.T && rtt_ij <= budget + g.T &&
+          !gs_lost_quiet(g, imp_loss, i, j, t0, GS_LK_PING, 0) && !gs_lost_quiet(g, imp_loss, j, i, t0, GS_LK_ACK, 0))
         success = true;
       if (success) {
         uint32_t aw = gs_meta_aw(m);
@@ -709,16 +727,16 @@ GS_DEV void gs_row_step(const GsDev& d, const GsGlobals& g, uint32_t i, uint32_t
       d.pass[i] = pass;
       if (target != GS_EMPTY32) {
         sink.stat(GS_ST_PROBES, 1);
-        bool ok = gs_key_truth(ktarget) == GS_TRUTH_UP && !gs_lost(g, sink, i, target, t, GS_LK_PING, 0) &&
-                  !gs_lost(g, sink, target, i, t, GS_LK_ACK, 0) &&
-                  gs_extra(g, i, target) + gs_extra(g, target, i) <= g.T;  // ack within ProbeTimeout
+        bool ok = gs_key_truth(ktarget) == GS_TRUTH_UP && !gs_lost(g, imp_loss, sink, i, target, t, GS_LK_PING, 0) &&
+                  !gs_lost(g, imp_loss, sink, target, i, t, GS_LK_ACK, 0) &&
+                  gs_extra(g, imp_delay, i, target) + gs_extra(g, imp_delay, target, i) <= g.T;  // ack within ProbeTimeout
         if (ok) {
           uint32_t aw = gs_meta_aw(m);
           m = gs_meta_set_aw(m, aw ? aw - 1u : 0u);
           due = t + g.P;
           sink.stat(GS_ST_ACKS, 1);
           if constexpr (Sink::kCoords) {  // the ack carries the peer's coordinate
-            if (d.coord != nullptr) gs_coord_on_ack(d.coord, d.ctag, d.adj, d.adj_idx, g, i, target, t);
+            if (d.coord != nullptr) gs_coord_on_ack(d.coord, d.ctag, d.adj, d.adj_idx, imp_delay, g, i, target, t);
           }
         } else {
           m = gs_meta_set_stage(m, GS_STAGE_WAIT_T);
@@ -788,8 +806,8 @@ GS_DEV void gs_row_step(const GsDev& d, const GsGlobals& g, uint32_t i, uint32_t
               pm &= pm - 1;
               if (sends[x] > q) pkt |= 1u << r;
             }
-            if (!gs_lost(g, sink, i, peers[q], t, GS_LK_GOSSIP, q))
-              gs_post(d, g, sink, (t + 1u + gs_extra(g, i, peers[q])) & g.ring_mask, peers[q], pkt);
+            if (!gs_lost(g, imp_loss, sink, i, peers[q], t, GS_LK_GOSSIP, q))
+              gs_post(d, g, sink, (t + 1u + gs_extra(g, imp_delay, i, peers[q])) & g.ring_mask, peers[q], pkt);
           }
           np = 0u;  // done: the general loop below has nothing left to do
         }
@@ -811,8 +829,8 @@ GS_DEV void gs_row_step(const GsDev& d, const GsGlobals& g, uint32_t i, uint32_t
           sink.stat(GS_ST_RUMORS_SENT, 1);
         }
         sink.stat(GS_ST_GOSSIP_PACKETS, 1);
-        if (!gs_lost(g, sink, i, peers[q], t, GS_LK_GOSSIP, q))
-          gs_post(d, g, sink, (t + 1u + gs_extra(g, i, peers[q])) & g.ring_mask, peers[q], pkt);
+        if (!gs_lost(g, imp_loss, sink, i, peers[q], t, GS_LK_GOSSIP, q))
+          gs_post(d, g, sink, (t + 1u + gs_extra(g, imp_delay, i, peers[q])) & g.ring_mask, peers[q], pkt);
       }
       if (queued != q0) d.queued[i] = queued;
     }
@@ -857,6 +875,13 @@ GS_DEV void gs_row_step(const GsDev& d, const GsGlobals& g, uint32_t i, uint32_t
     gs_post(d, g, sink, inxt, i, GS_WAKE_BIT);
 }
 
+template <class Sink>
+GS_DEV void gs_row_step(const GsDev& d, const GsGlobals& g, uint32_t i, uint32_t t, uint32_t gslot, uint32_t inb,
+                        Sink& sink) {
+  if (d.imp_loss != nullptr) gs_row_step_body<true>(d, g, i, t, gslot, inb, sink);
+  else gs_row_step_body<false>(d, g, i, t, gslot, inb, sink);
+}
+
 // ---------------------------------------------------------------------------------------
 // Staged fast path for the steady-state case of [U] memberlist.probe/probeNode: a member
 // with an empty mailbox whose probe ticker fires, whose ring cursor does not wrap and whose
@@ -880,7 +905,8 @@ GS_DEV void gs_fast_load(const GsDev& d, uint32_t cur, uint32_t i, GsFastProbe& 
 template <class G>
 GS_DEV bool gs_fast_target(const GsDev& d, const G& g, uint32_t cur, uint32_t i,
                            GsFastProbe& f) {
-  if (g.loss_thr != 0u || g.graph_n != 0u || d.coord != nullptr) return false;  // CSR rows, coordinates: generic path
+  if (g.loss_thr != 0u || g.graph_n != 0u || d.coord != nullptr || d.imp_loss != nullptr)
+    return false;  // CSR rows, coordinates, impaired members: generic path
   if (gs_key_truth(f.k) != GS_TRUTH_UP || gs_key_rank(f.k) != GS_RANK_ALIVE) return false;
   if (gs_meta_stage(f.m) != GS_STAGE_IDLE || (f.m & (GS_META_DIRTY | GS_META_ISOLATED))) return false;
   if (f.cursor >= g.n) return false;  // ring wrap: re-key in the generic path
@@ -903,7 +929,7 @@ GS_DEV bool gs_fast_finish(const GsDev& d, const G& g, Sink& sink, uint32_t i, u
   if (g.pp_interval != 0u && gs_pp_due(g.pp_interval, g.rot_pp, i / g.phase_group, t))
     return false;  // the push-pull ticker fires too: generic path
   uint32_t m = f.m;
-  if (gs_key_truth(f.kc) == GS_TRUTH_UP && gs_extra(g, i, f.c) + gs_extra(g, f.c, i) <= g.T) {
+  if (gs_key_truth(f.kc) == GS_TRUTH_UP && gs_extra(g, nullptr, i, f.c) + gs_extra(g, nullptr, f.c, i) <= g.T) {
     const uint32_t aw = gs_meta_aw(m);
     m = gs_meta_set_aw(m, aw ? aw - 1u : 0u);
     d.due[i] = t + g.P;

@@ -184,6 +184,24 @@ class Pool:
         assert m.ndim == 2 and m.shape[0] == m.shape[1]
         self._ck(self.lib.gsim_latency_set(self.h, m.shape[0], m.ctypes.data_as(C.POINTER(C.c_uint8))))
 
+    def impair(self, ids, loss_ppm: int, delay_ticks: int = 0):
+        """Degrade the listed members: UDP loss to and from each (ppm) and a receive delay (ticks);
+        (0, 0) clears it."""
+        arr = (C.c_uint32 * max(1, len(ids)))(*ids)
+        self._ck(self.lib.gsim_impair_many(self.h, arr, len(ids), loss_ppm, delay_ticks))
+
+    def impair_fraction(self, member_ppm: int, salt: int, loss_ppm: int, delay_ticks: int = 0) -> int:
+        """Degrade a seeded fraction (ppm) of the running members; returns how many were selected."""
+        out = C.c_uint32()
+        self._ck(self.lib.gsim_impair_fraction(self.h, member_ppm, salt, loss_ppm, delay_ticks, C.byref(out)))
+        return out.value
+
+    def impairment(self, member: int):
+        """(loss_ppm, delay_ticks) of one member, as set."""
+        loss, delay = C.c_uint32(), C.c_uint32()
+        self._ck(self.lib.gsim_impair_get(self.h, member, C.byref(loss), C.byref(delay)))
+        return loss.value, delay.value
+
     # -- time ---------------------------------------------------------------------
     def step(self, ticks: int = 1):
         self._ck(self.lib.gsim_step(self.h, ticks))

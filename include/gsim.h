@@ -272,6 +272,38 @@ int gsim_member_watch(gsim_pool* p, uint32_t id, int on);
  * n_dcs = 0 removes the matrix.  Callable between steps; packets in flight keep their slots. */
 int gsim_latency_set(gsim_pool* p, uint32_t n_dcs, const uint8_t* lat_ticks);
 
+/* Degraded members (simulator-only fault injection for Lifeguard experiments): member m has an
+ * impairment (loss_ppm[m], delay[m]), (0, 0) by default.
+ *  - Loss: a UDP packet from src to dst, whose Philox block r is the one the pool-wide loss draws
+ *    (r.x < packet_loss_ppm threshold), is also lost when r.y < thr(loss_ppm[src]) or
+ *    r.z < thr(loss_ppm[dst]), thr(ppm) = ppm * 2^32 / 1e6 (0xFFFFFFFF for 1e6).  A lost packet counts
+ *    once in GSIM_STAT_PACKETS_LOST.
+ *  - Receive delay: dst handles whatever it receives delay[dst] ticks late: a gossip packet sent at t
+ *    arrives at t + 1 + (latency matrix extra) + delay[dst]; a probe round trip i -> j -> i costs
+ *    delay[j] + delay[i] on top of the matrix, under the ProbeTimeout / indirect-stage / deadline rules of
+ *    gsim_latency_set.  Network coordinates measure it.
+ *  - Applies to gossip packets and to the probe / indirect-probe / nack / TCP-fallback legs; not to
+ *    push-pull (TCP), accusations or host operations.  An accused member learns of the accusation one tick
+ *    later without loss (one shared record per subject), so a degraded member that runs refutes and is
+ *    never declared Failed: what impairment measures is false suspicion, awareness and probe traffic.
+ *  - While any member is impaired the pool runs the generic per-member probe path (no probe fast paths,
+ *    no long or closed-form quiet windows); once every impairment is cleared it runs exactly like a pool
+ *    that never had one.
+ *  - Columns (4 + 1 bytes per member) are allocated by the first call that impairs somebody; members added
+ *    later start unimpaired.  Impairment is configuration: not part of gsim_state_hash; gsim_snapshot
+ *    carries it once the columns exist.  Single-GPU pools only (GSIM_ERR_STATE when sharded).
+ *  - GSIM_ERR_INVALID: loss_ppm > 1e6, or the largest latency-matrix extra + delay_ticks >
+ *    mailbox_depth - 2 (gsim_latency_set rejects a matrix that no longer fits the largest delay present).
+ *    GSIM_ERR_NOT_FOUND: an id that was never created. */
+/* Set the impairment of the listed members; (0, 0) clears it. */
+int gsim_impair_many(gsim_pool* p, const uint32_t* ids, size_t n, uint32_t loss_ppm, uint32_t delay_ticks);
+/* Impair every UP member i with philox(seed; i, salt, IMPAIR).x < member_ppm * 2^32 / 1e6 (a selection
+ * independent of gsim_crash_fraction's for the same salt); *n_impaired = members selected. */
+int gsim_impair_fraction(gsim_pool* p, uint32_t member_ppm, uint32_t salt, uint32_t loss_ppm, uint32_t delay_ticks,
+                         uint32_t* n_impaired);
+/* The impairment of member `id` exactly as it was set. */
+int gsim_impair_get(gsim_pool* p, uint32_t id, uint32_t* loss_ppm, uint32_t* delay_ticks);
+
 /* ---- time ---------------------------------------------------------------- */
 int gsim_step(gsim_pool* p, uint32_t ticks);
 #define GSIM_PRED_RUMOR_CONVERGED 1 /* arg = slot: every UP member heard it          */
