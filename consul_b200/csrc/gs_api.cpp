@@ -295,6 +295,11 @@ struct gsim_pool {
   uint32_t* imp_loss = nullptr;
   uint8_t* imp_delay = nullptr;
   uint32_t n_impaired = 0;
+  // host writes to device state not yet handed to the backend (see dev()), and whether handing an
+  // earlier batch over failed (reported by the API call it belonged to)
+  GsWriteBatch wb = {};
+  bool wb_failed = false;
+  uint32_t last_active = 0;  // GS_Q_LAST_ACTIVE as the last run_ticks left it (single-GPU pools)
 };
 
 static void counts_invalidate(gsim_pool* p) {
@@ -329,29 +334,71 @@ static int fail(gsim_pool* p, int code, const char* msg) {
   return code;
 }
 
+// ---- host writes to device state ------------------------------------------------------------
+// Queued as ops of one GsWriteBatch and handed to the backend, in order, right before the next thing
+// the host asks of the device (dev()) or at the end of the API call: a write costs no round trip, and
+// the read-modify-writes happen on the device, so the host never reads a word only to change it.
+static bool flush_writes(gsim_pool* p) {
+  if (!p->wb.n) return true;
+  const bool okk = p->be->write_batch(p->wb);
+  p->wb.n = 0;
+  if (!okk) p->wb_failed = true;
+  return okk;
+}
+
+// The backend, for anything that launches, copies or reads: every queued write comes before it.
+static GsBackend* dev(gsim_pool* p) {
+  flush_writes(p);
+  return p->be;
+}
+
+// End of an API call: its writes are on the stream, or the call fails.
+static int finish_writes(gsim_pool* p, int rc) {
+  const bool okk = flush_writes(p) && !p->wb_failed;
+  p->wb_failed = false;
+  if (!okk && rc == GSIM_OK) rc = fail(p, GSIM_ERR_CUDA, "device write batch");
+  return rc;
+}
+
+static bool put_op(gsim_pool* p, uint32_t op, const void* a, uint32_t v, const void* b = nullptr, uint32_t w = 0u,
+                   uint32_t x = 0u) {
+  mark_dirty(p);  // a host write to device state: whatever was known about quietness is void
+  if (p->wb.n == GS_WB_MAX && !flush_writes(p)) return false;
+  GsWriteOp& o = p->wb.op[p->wb.n++];
+  o.a = (uint64_t)(uintptr_t)a;
+  o.b = (uint64_t)(uintptr_t)b;
+  o.op = op;
+  o.v = v;
+  o.w = w;
+  o.x = x;
+  return true;
+}
+
 template <class T>
 static bool peek(gsim_pool* p, const T* col, size_t i, T* out) {
-  return p->be->d2h(out, col + i, sizeof(T));
+  return dev(p)->d2h(out, col + i, sizeof(T));
 }
 template <class T>
 static bool poke(gsim_pool* p, T* col, size_t i, T v) {
-  mark_dirty(p);  // a host write to device state: whatever was known about quietness is void
-  return p->be->h2d_word(col + i, &v, sizeof(T));
+  static_assert(sizeof(T) == 4 || sizeof(T) == 1, "device writes are words or bytes");
+  return put_op(p, sizeof(T) == 4 ? GS_WR_STORE32 : GS_WR_STORE8, col + i, (uint32_t)v);
 }
+static bool poke_or(gsim_pool* p, uint32_t* col, size_t i, uint32_t bits) { return put_op(p, GS_WR_OR32, col + i, bits); }
 
-// Host-side write of a member's key word: every replica on a sharded pool.
-static bool poke_key(gsim_pool* p, uint32_t buf, uint32_t i, uint32_t k) {
-  if (p->d.kst) {  // keep the member's status byte in step (see gs_kst_code)
-    uint8_t b;
-    if (!peek(p, p->d.kst, i, &b)) return false;
-    const uint32_t code = gs_kst_code(k);
-    b = (uint8_t)(buf ? ((b & 0x0Fu) | (code << 4)) : ((b & 0xF0u) | code));
-    if (!poke(p, p->d.kst, i, b)) return false;
-  }
-  if (!p->sharded) return poke(p, p->d.key[buf], i, k);
-  for (uint32_t r = 0; r < p->world; ++r)
-    if (!poke(p, p->d.key_rep[buf], (size_t)r * p->g.key_stride + i, k)) return false;
-  return true;
+// Host-side write of a member's key word (k, or the word AND k when and_mask): every replica on a
+// sharded pool, and the member's status byte in step (see gs_kst_code), derived on the device.
+static bool write_key(gsim_pool* p, uint32_t buf, uint32_t i, uint32_t k, bool and_mask) {
+  const uint32_t op = and_mask ? GS_WR_AND32 : GS_WR_STORE32;
+  for (uint32_t r = 0; r < (p->sharded ? p->world : 1u); ++r)
+    if (!put_op(p, op, p->d.key_rep[buf] + (size_t)r * p->g.key_stride + i, k)) return false;
+  return !p->d.kst || put_op(p, GS_WR_KST, p->d.kst + i, buf, p->d.key[buf] + i);
+}
+static bool poke_key(gsim_pool* p, uint32_t buf, uint32_t i, uint32_t k) { return write_key(p, buf, i, k, false); }
+
+// One more member has heard rumor r (`add` of them): heard_cnt[r] += add, and the rumor's convergence
+// tick is now if that makes every running member
+static bool heard_add(gsim_pool* p, uint32_t r, uint32_t add) {
+  return put_op(p, GS_WR_HEARD, p->d.heard_cnt + r, add, p->d.conv_tick + r, p->g.up_count, p->now);
 }
 
 // N-dependent scalars, recomputed whenever the member count changes (a11).
@@ -386,16 +433,18 @@ static void recompute_tables(gsim_pool* p) {
   p->g_dirty = true;
 }
 
+// Ordered before every later launch on the pool's stream, not waited for (the copy is staged).
 static bool upload_globals(gsim_pool* p) {
   if (!p->g_dirty) return true;
+  GsBackend* be = dev(p);
   if (p->sharded) {
     // the controller (rank 0) writes every rank's device copy; only `rank` differs
     for (uint32_t r = 0; r < p->world; ++r) {
       GsGlobals tmp = p->g;
       tmp.rank = r;
-      if (!p->be->h2d(p->pages + (size_t)r * GS_PAGE_BYTES + GS_PG_GLOBALS, &tmp, sizeof(GsGlobals))) return false;
+      if (!be->h2d_word(p->pages + (size_t)r * GS_PAGE_BYTES + GS_PG_GLOBALS, &tmp, sizeof(GsGlobals))) return false;
     }
-  } else if (!p->be->h2d(p->g_dev, &p->g, sizeof(GsGlobals))) {
+  } else if (!be->h2d_word(p->g_dev, &p->g, sizeof(GsGlobals))) {
     return false;
   }
   p->g_dirty = false;
@@ -418,7 +467,7 @@ struct BlobHdr {
 
 template <class F>
 static int controller_call(gsim_pool* p, void* out, size_t out_bytes, F f) {
-  if (!p->sharded) return f();
+  if (!p->sharded) return finish_writes(p, f());
   const uint32_t seq = p->call_seq++;
   const uint32_t slot = seq & 1u;
   uint8_t* blob_dev = p->pages + GS_PG_BLOB + (size_t)slot * GS_BLOB_BYTES;  // in rank 0's page
@@ -426,7 +475,7 @@ static int controller_call(gsim_pool* p, void* out, size_t out_bytes, F f) {
   BlobHdr h;
   memset(&h, 0, sizeof(h));
   if (p->rank == 0) {
-    h.rc = f();
+    h.rc = finish_writes(p, f());  // (the blob copy below waits for them: done before any rank goes on)
     if (p->g_dirty && !upload_globals(p)) h.rc = h.rc ? h.rc : GSIM_ERR_CUDA;
     h.now = p->now;
     h.n_established = p->n_established;
@@ -451,12 +500,12 @@ static int controller_call(gsim_pool* p, void* out, size_t out_bytes, F f) {
     w += h.n_sched * sizeof(Sched);
     if (out && h.out_bytes) memcpy(w, out, h.out_bytes);
     w += h.out_bytes;
-    if (!p->be->h2d(blob_dev, blob.data(), (size_t)(w - blob.data()))) return fail(p, GSIM_ERR_CUDA, "blob h2d");
-    if (!p->be->xbar_host(p->xb)) return fail(p, GSIM_ERR_CUDA, "barrier");
+    if (!dev(p)->h2d(blob_dev, blob.data(), (size_t)(w - blob.data()))) return fail(p, GSIM_ERR_CUDA, "blob h2d");
+    if (!dev(p)->xbar_host(p->xb)) return fail(p, GSIM_ERR_CUDA, "barrier");
     return h.rc;
   }
-  if (!p->be->xbar_host(p->xb)) return fail(p, GSIM_ERR_CUDA, "barrier");
-  if (!p->be->d2h(blob.data(), blob_dev, GS_BLOB_BYTES)) return fail(p, GSIM_ERR_CUDA, "blob d2h");
+  if (!dev(p)->xbar_host(p->xb)) return fail(p, GSIM_ERR_CUDA, "barrier");
+  if (!dev(p)->d2h(blob.data(), blob_dev, GS_BLOB_BYTES)) return fail(p, GSIM_ERR_CUDA, "blob d2h");
   const uint8_t* r = blob.data();
   memcpy(&h, r, sizeof(h)); r += sizeof(h);
   if (h.call_seq != seq || h.want_bytes != (uint32_t)out_bytes) {
@@ -509,7 +558,7 @@ static void rebuild_class_masks(gsim_pool* p) {
 
 template <class T>
 static bool alloc_col(gsim_pool* p, T** out, size_t count) {
-  void* q = p->be->alloc(count * sizeof(T));
+  void* q = dev(p)->alloc(count * sizeof(T));
   if (!q) return false;
   p->allocs.push_back(q);
   *out = reinterpret_cast<T*>(q);
@@ -524,9 +573,9 @@ static bool reset_tick_flags(gsim_pool* p) {
   const uint32_t zero = 0;
   for (uint32_t r = 0; r < p->world; ++r) {
     uint8_t* page = p->pages + (size_t)r * GS_PAGE_BYTES;
-    if (!p->be->h2d(page + GS_PG_TICK_FLAGS, words, sizeof(words))) return false;
-    if (!p->be->h2d(page + GS_PG_DONE_CTR, &zero, 4)) return false;
-    if (!p->be->h2d(page + GS_PG_TICK_BASE, &p->now, 4)) return false;
+    if (!dev(p)->h2d(page + GS_PG_TICK_FLAGS, words, sizeof(words))) return false;
+    if (!dev(p)->h2d(page + GS_PG_DONE_CTR, &zero, 4)) return false;
+    if (!dev(p)->h2d(page + GS_PG_TICK_BASE, &p->now, 4)) return false;
   }
   return true;
 }
@@ -535,7 +584,7 @@ static bool reset_tick_flags(gsim_pool* p) {
 static bool reset_qstate(gsim_pool* p) {
   const uint32_t words[GS_Q_WORDS] = {p->now, GS_NEVER, p->now, 0u};  // last-active+1 = now: tick now-1 counts as active
   for (uint32_t r = 0; r < (p->sharded ? p->world : 1u); ++r)
-    if (!p->be->h2d(p->d.qstate[r], words, sizeof(words))) return false;
+    if (!dev(p)->h2d(p->d.qstate[r], words, sizeof(words))) return false;
   mark_dirty(p);
   return true;
 }
@@ -543,7 +592,7 @@ static bool reset_qstate(gsim_pool* p) {
 // Device-side initial state: empty columns, zeroed counters, the converged initial members.
 // On a sharded pool this runs on rank 0 only and reaches every GPU through the unified columns.
 static int init_device_state(gsim_pool* p) {
-  GsBackend* be = p->be;
+  GsBackend* be = dev(p);
   GsDev& d = p->d;
   GsGlobals& g = p->g;
   const size_t cap = g.cap;
@@ -828,7 +877,7 @@ extern "C" int gsim_shard_export_fds(gsim_pool* p, int* fds, size_t cap, size_t*
 extern "C" int gsim_shard_attach(gsim_pool* p, uint32_t peer_rank, const int* fds, size_t n) {
   if (!p || !p->sharded || p->ready || !fds) return GSIM_ERR_INVALID;
   std::lock_guard<std::mutex> lk(p->mu);
-  if (!p->be->shard_attach(peer_rank, fds, n)) return fail(p, GSIM_ERR_CUDA, "shard_attach");
+  if (!dev(p)->shard_attach(peer_rank, fds, n)) return fail(p, GSIM_ERR_CUDA, "shard_attach");
   p->attached += 1;
   return GSIM_OK;
 }
@@ -839,7 +888,7 @@ extern "C" int gsim_shard_ready(gsim_pool* p) {
   std::lock_guard<std::mutex> lk(p->mu);
   if (p->ready) return GSIM_OK;
   if (p->attached != p->world) return fail(p, GSIM_ERR_STATE, "not every peer rank has been attached");
-  if (!p->be->xbar_host(p->xb)) return fail(p, GSIM_ERR_CUDA, "barrier");  // every page is mapped and zeroed
+  if (!dev(p)->xbar_host(p->xb)) return fail(p, GSIM_ERR_CUDA, "barrier");  // every page is mapped and zeroed
   int rc = controller_call(p, nullptr, 0, [&]() -> int { return init_device_state(p); });
   if (rc) return fail(p, rc, "init");
   p->ready = true;
@@ -849,11 +898,11 @@ extern "C" int gsim_shard_ready(gsim_pool* p) {
 extern "C" void gsim_pool_destroy(gsim_pool* p) {
   if (!p) return;
   if (p->be) {
-    p->be->sync();
-    if (p->stage) p->be->host_free(p->stage);
+    dev(p)->sync();
+    if (p->stage) dev(p)->host_free(p->stage);
     delete p->workers;
     p->workers = nullptr;
-    for (void* q : p->allocs) p->be->release(q);
+    for (void* q : p->allocs) dev(p)->release(q);
     delete p->be;
   }
   delete p;
@@ -883,9 +932,9 @@ static int collective_recount(gsim_pool* p) {
   shard_rows(p, &first, &count);
   // (the device copy of the globals is current: every controller call ends with the upload)
   const bool usable = !(p->rank == 0 && p->g_dirty);
-  if (!p->be->recount(p->d, p->g_dev, p->g, p->now, first, count, &part)) return GSIM_ERR_CUDA;
-  if (!p->be->h2d(p->pages + GS_PG_SCRATCH + 512u * p->rank, &part, sizeof(part))) return GSIM_ERR_CUDA;
-  if (!p->be->xbar_host(p->xb)) return GSIM_ERR_CUDA;
+  if (!dev(p)->recount(p->d, p->g_dev, p->g, p->now, first, count, &part)) return GSIM_ERR_CUDA;
+  if (!dev(p)->h2d(p->pages + GS_PG_SCRATCH + 512u * p->rank, &part, sizeof(part))) return GSIM_ERR_CUDA;
+  if (!dev(p)->xbar_host(p->xb)) return GSIM_ERR_CUDA;
   if (p->rank == 0) {
     p->partials_fresh = usable;
     p->partials_seq = p->dirty_seq;
@@ -899,7 +948,7 @@ static bool do_recount(gsim_pool* p) {
   if (!upload_globals(p)) return false;
   if (p->sharded && p->partials_fresh && p->partials_seq == p->dirty_seq && p->partials_now == p->now) {
     std::vector<uint8_t> raw(512u * p->world);
-    if (!p->be->d2h(raw.data(), p->pages + GS_PG_SCRATCH, raw.size())) return false;
+    if (!dev(p)->d2h(raw.data(), p->pages + GS_PG_SCRATCH, raw.size())) return false;
     memset(&p->rc, 0, sizeof(p->rc));
     uint32_t* sum = reinterpret_cast<uint32_t*>(&p->rc);
     for (uint32_t r = 0; r < p->world; ++r) {
@@ -908,7 +957,7 @@ static bool do_recount(gsim_pool* p) {
       const uint32_t* w = reinterpret_cast<const uint32_t*>(&part);
       for (size_t x = 0; x < sizeof(GsRecount) / 4; ++x) sum[x] += w[x];
     }
-  } else if (!p->be->recount(p->d, p->g_dev, p->g, p->now, 0u, p->g.n, &p->rc)) {
+  } else if (!dev(p)->recount(p->d, p->g_dev, p->g, p->now, 0u, p->g.n, &p->rc)) {
     return false;
   }
   p->counts_stale = false;
@@ -917,29 +966,33 @@ static bool do_recount(gsim_pool* p) {
 
 static bool and_bit_columns(gsim_pool* p, uint32_t keep);
 
-static int retire_slot(gsim_pool* p, uint32_t slot) {
+// Free a rumor slot, all but clearing its bits from the heard / queued / mailbox columns (the caller
+// does that, for every slot it frees at once: and_bit_columns).
+static int release_slot(gsim_pool* p, uint32_t slot) {
   GsGlobals& g = p->g;
   GsRumor& ru = g.rumors[slot];
   if (ru.kind == GSIM_RUMOR_ALIVE) {
-    // fold into the base state: the subject becomes known to every non-isolated member
-    uint32_t k0, k1;
-    if (!peek(p, p->d.key[0], ru.subject, &k0) || !peek(p, p->d.key[1], ru.subject, &k1))
-      return GSIM_ERR_CUDA;
-    if (gs_key_pending(k0)) p->n_established += 1;
-    k0 &= ~(1u << 4);
-    k1 &= ~(1u << 4);
-    if (!poke_key(p, 0, ru.subject, k0) || !poke_key(p, 1, ru.subject, k1))
+    // fold into the base state: the subject becomes known to every non-isolated member.  The subject
+    // of a tracked alive rumor is pending in both key buffers: gsim_member_add sets the bit, nothing
+    // but this clears it, and reaping or pruning a member keeps it.
+    p->n_established += 1;
+    if (!write_key(p, 0, ru.subject, ~(1u << 4), true) || !write_key(p, 1, ru.subject, ~(1u << 4), true))
       return GSIM_ERR_CUDA;
   }
   g.active_mask &= ~(1u << slot);
   memset(&ru, 0, sizeof(ru));
   p->rh[slot] = RumorHost();
   rebuild_class_masks(p);
-  if (!and_bit_columns(p, ~(1u << slot))) return GSIM_ERR_CUDA;
   if (!poke(p, p->d.heard_cnt, slot, 0u) || !poke(p, p->d.conv_tick, slot, GS_EMPTY32))
     return GSIM_ERR_CUDA;
   counts_invalidate(p);
   return GSIM_OK;
+}
+
+static int retire_slot(gsim_pool* p, uint32_t slot) {
+  const int rc = release_slot(p, slot);
+  if (rc) return rc;
+  return and_bit_columns(p, ~(1u << slot)) ? GSIM_OK : GSIM_ERR_CUDA;
 }
 
 // heard/queued/inbox bits of a freed slot must be zero before the slot is reused.
@@ -949,7 +1002,7 @@ static bool and_bit_columns(gsim_pool* p, uint32_t keep) {
     p->pending_keep &= keep;
     return true;
   }
-  return p->be->and_columns(p->d, p->g, keep, 0u, p->g.n);
+  return dev(p)->and_columns(p->d, p->g, keep, 0u, p->g.n);
 }
 
 // ... which is this, on every rank, right after the controller call that collected the mask.
@@ -957,10 +1010,10 @@ static int apply_pending_and(gsim_pool* p) {
   if (!p->sharded || p->pending_keep == 0xFFFFFFFFu) return GSIM_OK;
   uint32_t first, count;
   shard_rows(p, &first, &count);
-  const bool ok = p->be->and_columns(p->d, p->g, p->pending_keep, first, count) && p->be->sync();
+  const bool ok = dev(p)->and_columns(p->d, p->g, p->pending_keep, first, count) && dev(p)->sync();
   p->pending_keep = 0xFFFFFFFFu;
   // nobody goes on (to reuse a freed slot, to tick) before every rank's rows are clean
-  if (!ok || !p->be->xbar_host(p->xb)) return GSIM_ERR_CUDA;
+  if (!ok || !dev(p)->xbar_host(p->xb)) return GSIM_ERR_CUDA;
   return GSIM_OK;
 }
 
@@ -973,16 +1026,20 @@ static int auto_retire(gsim_pool* p) {
     if (((g.active_mask >> r) & 1u) && g.rumors[r].kind != GSIM_RUMOR_USER_EVENT) cand |= 1u << r;
   if (!cand) return GSIM_OK;
   if (!do_recount(p)) return GSIM_ERR_CUDA;
+  uint32_t keep = 0xFFFFFFFFu;
   for (uint32_t r = 0; r < GS_MAX_RUMORS; ++r) {
     if (!((cand >> r) & 1u)) continue;
     // an alive rumor folds into the base set only when nobody still depends on having
     // heard it individually (members that have not joined the base set yet)
     if (g.rumors[r].kind == GSIM_RUMOR_ALIVE && p->rc.isolated_up != 0) continue;
     if (p->rc.heard_cnt[r] == g.up_count && p->rc.queued_cnt[r] == 0) {
-      int rcode = retire_slot(p, r);
+      int rcode = release_slot(p, r);
       if (rcode) return rcode;
+      keep &= ~(1u << r);
     }
   }
+  // one pass over the bit columns for every slot freed
+  if (keep != 0xFFFFFFFFu && !and_bit_columns(p, keep)) return GSIM_ERR_CUDA;
   return GSIM_OK;
 }
 
@@ -1005,10 +1062,7 @@ static int alloc_slot(gsim_pool* p, uint32_t* slot_out) {
 // A member whose broadcast queue became non-empty between ticks must be looked at by the
 // next tick: set the wake bit in the mailbox that tick will read.
 static bool post_wake(gsim_pool* p, uint32_t row) {
-  uint32_t* col = p->d.inbox[p->now & p->g.ring_mask];
-  uint32_t w;
-  if (!peek(p, col, row, &w)) return false;
-  return poke(p, col, row, w | GS_WAKE_BIT);
+  return poke_or(p, p->d.inbox[p->now & p->g.ring_mask], row, GS_WAKE_BIT);
 }
 
 // ---- message sizes: what the encoder (gs_wire.h) produces for this member ------------------------
@@ -1044,11 +1098,7 @@ static int start_rumor(gsim_pool* p, uint32_t slot, uint32_t kind, uint32_t subj
   g.active_mask |= 1u << slot;
   rebuild_class_masks(p);
   // the origin holds it with transmits = 0
-  uint32_t h, q;
-  if (!peek(p, p->d.heard, origin, &h) || !peek(p, p->d.queued, origin, &q)) return GSIM_ERR_CUDA;
-  h |= 1u << slot;
-  q |= 1u << slot;
-  if (!poke(p, p->d.heard, origin, h) || !poke(p, p->d.queued, origin, q)) return GSIM_ERR_CUDA;
+  if (!poke_or(p, p->d.heard, origin, 1u << slot) || !poke_or(p, p->d.queued, origin, 1u << slot)) return GSIM_ERR_CUDA;
   if (!poke(p, p->d.tx, GS_TX(slot, g.cap, origin), (uint8_t)0)) return GSIM_ERR_CUDA;
   if (!post_wake(p, origin)) return GSIM_ERR_CUDA;
   if (!poke(p, p->d.heard_cnt, slot, 1u)) return GSIM_ERR_CUDA;
@@ -1060,15 +1110,15 @@ static int start_rumor(gsim_pool* p, uint32_t slot, uint32_t kind, uint32_t subj
 static void log_host_event(gsim_pool* p, uint32_t type, uint32_t subject, uint32_t observer,
                            uint32_t ltime) {
   uint32_t cur[2];
-  if (!p->be->d2h(cur, p->d.evlog_cursor, 8)) return;
+  if (!dev(p)->d2h(cur, p->d.evlog_cursor, 8)) return;
   if (cur[0] < p->g.evlog_cap) {
     GsEventRec e = {p->now, type, subject, observer, ltime, 0u};
-    p->be->h2d(p->d.evlog + cur[0], &e, sizeof(e));
+    dev(p)->h2d(p->d.evlog + cur[0], &e, sizeof(e));
     cur[0]++;
   } else {
     cur[1]++;
   }
-  p->be->h2d(p->d.evlog_cursor, cur, 8);
+  dev(p)->h2d(p->d.evlog_cursor, cur, 8);
 }
 
 // ---- membership operations -------------------------------------------------------
@@ -1084,16 +1134,15 @@ extern "C" int gsim_member_add(gsim_pool* p, const gsim_member_desc* desc, uint3
   if (rc) return fail(p, rc, "no free rumor slot for the member's alive broadcast");
   const uint32_t id = g.n;
   if (!upload_globals(p)) return fail(p, GSIM_ERR_CUDA, "upload");
-  if (!p->be->init_rows(p->d, p->g_dev, g, id, 1, p->now)) return fail(p, GSIM_ERR_CUDA, "init_rows");
+  if (!dev(p)->init_rows(p->d, p->g_dev, g, id, 1, p->now)) return fail(p, GSIM_ERR_CUDA, "init_rows");
   // [U] memberlist.Create -> setAlive: incarnation 1, alive{} queued on the new member;
   // pending: other members learn of it only through that rumor (aliveNode).
   const uint32_t k = gs_key_make(1u, 1u, GS_RANK_ALIVE, GS_TRUTH_UP);
-  uint32_t m;
-  if (!peek(p, p->d.meta, id, &m)) return fail(p, GSIM_ERR_CUDA, "peek");
+  uint32_t flags = 0;
   // it knows nobody yet; with an empty base set there is nothing it could be missing
-  if (p->n_established > 0) m |= GS_META_ISOLATED;
-  if (desc && (desc->flags & GSIM_MEMBER_WATCHED)) m |= GS_META_WATCHED;
-  if (!poke_key(p, 0, id, k) || !poke_key(p, 1, id, k) || !poke(p, p->d.meta, id, m))
+  if (p->n_established > 0) flags |= GS_META_ISOLATED;
+  if (desc && (desc->flags & GSIM_MEMBER_WATCHED)) flags |= GS_META_WATCHED;
+  if (!poke_key(p, 0, id, k) || !poke_key(p, 1, id, k) || (flags && !poke_or(p, p->d.meta, id, flags)))
     return fail(p, GSIM_ERR_CUDA, "poke");
   g.n += 1;
   g.up_count += 1;
@@ -1109,10 +1158,10 @@ extern "C" int gsim_member_add(gsim_pool* p, const gsim_member_desc* desc, uint3
 
 // One direction of a join push-pull: `dst` merges what `src` knows
 // ([U] memberlist.mergeState -> aliveNode; [U] serf/delegate.go MergeRemoteState).
-static int merge_remote(gsim_pool* p, uint32_t dst, uint32_t src, bool ignore_old_events) {
+// rs / rd: the rows of both ends as rows_read gave them, brought up to date with every write of the
+// join so far; rd gets this merge's writes.
+static int merge_remote(gsim_pool* p, uint32_t dst, const uint32_t* rs, uint32_t* rd, bool ignore_old_events) {
   GsGlobals& g = p->g;
-  uint32_t rs[8], rd[8];  // {key0, key1, meta, heard, queued, ltime_member, ltime_event, event_min} of both ends
-  if (!p->be->row_read(p->d, src, rs) || !p->be->row_read(p->d, dst, rd)) return GSIM_ERR_CUDA;
   uint32_t hs = rs[3], hd = rd[3], qd = rd[4], lm_s = rs[5], le_s = rs[6], lm_d = rd[5], le_d = rd[6], emin = rd[7], md = rd[2];
   // clocks: Witness(remote - 1)  ==  max(local, remote)
   if (lm_s > lm_d) lm_d = lm_s;
@@ -1138,16 +1187,7 @@ static int merge_remote(gsim_pool* p, uint32_t dst, uint32_t src, bool ignore_ol
     }
     if (accept) {
       accepted |= 1u << r;
-      if (!poke(p, p->d.tx, GS_TX(r, g.cap, dst), (uint8_t)0)) return GSIM_ERR_CUDA;
-      uint32_t c;
-      if (!peek(p, p->d.heard_cnt, r, &c)) return GSIM_ERR_CUDA;
-      c += 1;
-      if (!poke(p, p->d.heard_cnt, r, c)) return GSIM_ERR_CUDA;
-      if (c == g.up_count) {
-        uint32_t ct;
-        if (!peek(p, p->d.conv_tick, r, &ct)) return GSIM_ERR_CUDA;
-        if (ct == GS_EMPTY32 && !poke(p, p->d.conv_tick, r, p->now)) return GSIM_ERR_CUDA;
-      }
+      if (!poke(p, p->d.tx, GS_TX(r, g.cap, dst), (uint8_t)0) || !heard_add(p, r, 1u)) return GSIM_ERR_CUDA;
     }
   }
   hd |= accepted;
@@ -1157,6 +1197,11 @@ static int merge_remote(gsim_pool* p, uint32_t dst, uint32_t src, bool ignore_ol
       !poke(p, p->d.ltime_member, dst, lm_d) || !poke(p, p->d.ltime_event, dst, le_d) ||
       !poke(p, p->d.event_min, dst, emin))
     return GSIM_ERR_CUDA;
+  rd[3] = hd;
+  rd[4] = qd;
+  rd[5] = lm_d;
+  rd[6] = le_d;
+  rd[7] = emin;
   counts_invalidate(p);
   return GSIM_OK;
 }
@@ -1170,32 +1215,39 @@ extern "C" int gsim_join(gsim_pool* p, uint32_t id, const uint32_t* seeds, size_
   return controller_call(p, n_ok, sizeof(int), [&]() -> int {
   GsGlobals& g = p->g;
   if (id >= g.n) return fail(p, GSIM_ERR_NOT_FOUND, "unknown member");
-  uint32_t kid;
-  if (!peek(p, p->d.key[p->now & 1u], id, &kid)) return fail(p, GSIM_ERR_CUDA, "peek");
-  if (gs_key_truth(kid) != GS_TRUTH_UP) return fail(p, GSIM_ERR_STATE, "member is not running");
+  // the joiner's and every seed's row in one round trip; the join works on this copy from here on,
+  // writing to it what it writes to the device
+  std::vector<uint32_t> ids(1, id);
+  for (size_t s = 0; s < n_seeds; ++s)
+    if (seeds[s] < g.n && std::find(ids.begin(), ids.end(), seeds[s]) == ids.end()) ids.push_back(seeds[s]);
+  std::vector<uint32_t> rows(ids.size() * 8);
+  if (!dev(p)->rows_read(p->d, ids.data(), (uint32_t)ids.size(), rows.data())) return fail(p, GSIM_ERR_CUDA, "rows_read");
+  auto row = [&](uint32_t m) { return rows.data() + 8 * (std::find(ids.begin(), ids.end(), m) - ids.begin()); };
+  const uint32_t cur = p->now & 1u;  // (rows hold key[0] and key[1])
+  uint32_t* ri = row(id);
+  if (gs_key_truth(ri[cur]) != GS_TRUTH_UP) return fail(p, GSIM_ERR_STATE, "member is not running");
   int okc = 0;
   for (size_t s = 0; s < n_seeds; ++s) {
     uint32_t sd = seeds[s];
     if (sd >= g.n || sd == id) continue;
-    uint32_t ks;
-    if (!peek(p, p->d.key[p->now & 1u], sd, &ks)) return fail(p, GSIM_ERR_CUDA, "peek");
-    if (gs_key_truth(ks) != GS_TRUTH_UP) continue;  // unreachable seed: Join skips it
+    uint32_t* rsd = row(sd);
+    if (gs_key_truth(rsd[cur]) != GS_TRUTH_UP) continue;  // unreachable seed: Join skips it
     // push-pull in both directions; eventJoinIgnore applies to the joiner only
-    int rc = merge_remote(p, id, sd, ignore_old != 0);
-    if (!rc) rc = merge_remote(p, sd, id, false);
+    int rc = merge_remote(p, id, rsd, ri, ignore_old != 0);
+    if (!rc) rc = merge_remote(p, sd, ri, rsd, false);
     if (rc) return fail(p, rc, "merge");
-    uint32_t mi, ms;
-    if (!peek(p, p->d.meta, id, &mi) || !peek(p, p->d.meta, sd, &ms)) return fail(p, GSIM_ERR_CUDA, "peek");
+    uint32_t mi = ri[2], ms = rsd[2];
     uint32_t iso = mi & ms & GS_META_ISOLATED;
     mi = (mi & ~GS_META_ISOLATED) | iso;
     ms = (ms & ~GS_META_ISOLATED) | iso;
     if (!poke(p, p->d.meta, id, mi) || !poke(p, p->d.meta, sd, ms)) return fail(p, GSIM_ERR_CUDA, "poke");
+    ri[2] = mi;
+    rsd[2] = ms;
     ++okc;
   }
   if (okc > 0) {
     // [U] serf.Join -> broadcastJoin(clock.Time()): Witness(ltime), join intent queued
-    uint32_t lm;
-    if (!peek(p, p->d.ltime_member, id, &lm)) return fail(p, GSIM_ERR_CUDA, "peek");
+    const uint32_t lm = ri[5];
     uint32_t slot;
     int rc = alloc_slot(p, &slot);
     if (rc == GSIM_OK) {
@@ -1235,11 +1287,7 @@ static int refresh_after_truth_change(gsim_pool* p) {
   for (uint32_t r = 0; r < GS_MAX_RUMORS; ++r) {
     if (!((g.active_mask >> r) & 1u)) continue;
     if (!poke(p, p->d.heard_cnt, r, p->rc.heard_cnt[r])) return GSIM_ERR_CUDA;
-    if (p->rc.heard_cnt[r] == g.up_count) {
-      uint32_t ct;
-      if (!peek(p, p->d.conv_tick, r, &ct)) return GSIM_ERR_CUDA;
-      if (ct == GS_EMPTY32 && !poke(p, p->d.conv_tick, r, p->now)) return GSIM_ERR_CUDA;
-    }
+    if (p->rc.heard_cnt[r] == g.up_count && !heard_add(p, r, 0u)) return GSIM_ERR_CUDA;  // (converged now?)
   }
   return GSIM_OK;
 }
@@ -1273,7 +1321,7 @@ extern "C" int gsim_crash_fraction(gsim_pool* p, uint32_t ppm, uint32_t salt, ui
   uint32_t cnt = 0;
   if (!upload_globals(p)) return fail(p, GSIM_ERR_CUDA, "upload");
   mark_dirty(p);
-  if (!p->be->crash_fraction(p->d, p->g_dev, p->g, thr, salt, p->now, &cnt))
+  if (!dev(p)->crash_fraction(p->d, p->g_dev, p->g, thr, salt, p->now, &cnt))
     return fail(p, GSIM_ERR_CUDA, "crash_fraction");
   if (n_crashed) *n_crashed = cnt;
   int rc = refresh_after_truth_change(p);
@@ -1416,12 +1464,7 @@ extern "C" int gsim_user_event(gsim_pool* p, uint32_t id, const void* name, size
       uint32_t h, q;
       if (!peek(p, p->d.heard, id, &h) || !peek(p, p->d.queued, id, &q)) return fail(p, GSIM_ERR_CUDA, "peek");
       if (!((h >> r) & 1u)) {
-        uint32_t c, ct;
-        if (!poke(p, p->d.heard, id, h | (1u << r)) || !peek(p, p->d.heard_cnt, r, &c) ||
-            !poke(p, p->d.heard_cnt, r, c + 1u) || !peek(p, p->d.conv_tick, r, &ct))
-          return fail(p, GSIM_ERR_CUDA, "poke");
-        if (c + 1u == g.up_count && ct == GS_EMPTY32 && !poke(p, p->d.conv_tick, r, p->now))
-          return fail(p, GSIM_ERR_CUDA, "poke");
+        if (!poke(p, p->d.heard, id, h | (1u << r)) || !heard_add(p, r, 1u)) return fail(p, GSIM_ERR_CUDA, "poke");
         if (m & GS_META_WATCHED) log_host_event(p, GSIM_EVENT_USER, r, id, le);
       }
       if (!poke(p, p->d.queued, id, q | (1u << r)) || !poke(p, p->d.tx, GS_TX(r, g.cap, id), (uint8_t)0) ||
@@ -1491,13 +1534,8 @@ extern "C" int gsim_rumor_inject(gsim_pool* p, uint32_t slot, uint32_t id, int* 
     if (m & GS_META_WATCHED) log_host_event(p, GSIM_EVENT_MEMBER_UPDATE, ru.subject, id, 0u);
   }
   if (!accept) return GSIM_OK;
-  uint32_t c, ct;
   if (!poke(p, p->d.heard, id, h | (1u << slot)) || !poke(p, p->d.queued, id, q | (1u << slot)) ||
-      !poke(p, p->d.tx, GS_TX(slot, g.cap, id), (uint8_t)0) || !post_wake(p, id) ||
-      !peek(p, p->d.heard_cnt, slot, &c) || !poke(p, p->d.heard_cnt, slot, c + 1u) ||
-      !peek(p, p->d.conv_tick, slot, &ct))
-    return fail(p, GSIM_ERR_CUDA, "poke");
-  if (c + 1u == g.up_count && ct == GS_EMPTY32 && !poke(p, p->d.conv_tick, slot, p->now))
+      !poke(p, p->d.tx, GS_TX(slot, g.cap, id), (uint8_t)0) || !post_wake(p, id) || !heard_add(p, slot, 1u))
     return fail(p, GSIM_ERR_CUDA, "poke");
   counts_invalidate(p);
   *accepted_out = 1;
@@ -1533,7 +1571,7 @@ extern "C" int gsim_graph_set(gsim_pool* p, uint32_t n_rows, const uint32_t* row
   uint32_t *rp_dev = nullptr, *col_dev = nullptr;
   if (!alloc_col(p, &rp_dev, (size_t)n_rows + 1) || !alloc_col(p, &col_dev, (size_t)(nnz ? nnz : 1)))
     return fail(p, GSIM_ERR_NOMEM, "graph allocation");
-  if (!p->be->h2d(rp_dev, row_ptr, ((size_t)n_rows + 1) * 4) || (nnz && !p->be->h2d(col_dev, col_idx, (size_t)nnz * 4)))
+  if (!dev(p)->h2d(rp_dev, row_ptr, ((size_t)n_rows + 1) * 4) || (nnz && !dev(p)->h2d(col_dev, col_idx, (size_t)nnz * 4)))
     return fail(p, GSIM_ERR_CUDA, "h2d");
   p->graph_rp.assign(row_ptr, row_ptr + n_rows + 1);
   p->graph_col.assign(col_idx, col_idx + nnz);
@@ -1616,7 +1654,7 @@ static bool impair_max_delay(gsim_pool* p, uint32_t* out) {
   *out = 0;
   if (!p->imp_delay || !p->g.n) return true;
   std::vector<uint8_t> v(p->g.n);
-  if (!p->be->d2h(v.data(), p->imp_delay, v.size())) return false;
+  if (!dev(p)->d2h(v.data(), p->imp_delay, v.size())) return false;
   for (uint8_t x : v) *out = x > *out ? x : *out;
   return true;
 }
@@ -1627,7 +1665,7 @@ static bool impair_alloc(gsim_pool* p) {
   uint32_t* loss = nullptr;
   uint8_t* delay = nullptr;
   if (!alloc_col(p, &loss, cap) || !alloc_col(p, &delay, cap)) return false;
-  if (!p->be->fill32(loss, 0, cap) || !p->be->fill8(delay, 0, cap)) return false;
+  if (!dev(p)->fill32(loss, 0, cap) || !dev(p)->fill8(delay, 0, cap)) return false;
   p->imp_loss = loss;
   p->imp_delay = delay;
   return true;
@@ -1646,7 +1684,7 @@ static bool impair_recount(gsim_pool* p) {
   if (p->imp_loss && p->g.n) {
     std::vector<uint32_t> loss(p->g.n);
     std::vector<uint8_t> delay(p->g.n);
-    if (!p->be->d2h(loss.data(), p->imp_loss, loss.size() * 4) || !p->be->d2h(delay.data(), p->imp_delay, delay.size()))
+    if (!dev(p)->d2h(loss.data(), p->imp_loss, loss.size() * 4) || !dev(p)->d2h(delay.data(), p->imp_delay, delay.size()))
       return false;
     for (uint32_t i = 0; i < p->g.n; ++i) p->n_impaired += (loss[i] | delay[i]) != 0u ? 1u : 0u;
   }
@@ -1698,7 +1736,7 @@ extern "C" int gsim_impair_fraction(gsim_pool* p, uint32_t member_ppm, uint32_t 
   if (!upload_globals(p)) return fail(p, GSIM_ERR_CUDA, "upload");
   const uint32_t thr = ppm_to_thr(loss_ppm);
   uint32_t counts[2] = {0, 0};
-  if (!p->be->impair_fraction(p->d, p->g_dev, p->g, p->imp_loss, p->imp_delay, ppm_to_thr(member_ppm), salt, thr,
+  if (!dev(p)->impair_fraction(p->d, p->g_dev, p->g, p->imp_loss, p->imp_delay, ppm_to_thr(member_ppm), salt, thr,
                               delay_ticks, counts))
     return fail(p, GSIM_ERR_CUDA, "impair_fraction");
   p->n_impaired = p->n_impaired - counts[1] + (thr != 0u || delay_ticks != 0u ? counts[0] : 0u);
@@ -1809,7 +1847,7 @@ static int reap_pass(gsim_pool* p) {
   uint32_t counts[2] = {0, 0};
   if (!upload_globals(p)) return GSIM_ERR_CUDA;
   mark_dirty(p);
-  if (!p->be->reap_rows(p->d, p->g_dev, p->g, p->now, r.reconnect, r.tombstone,
+  if (!dev(p)->reap_rows(p->d, p->g_dev, p->g, p->now, r.reconnect, r.tombstone,
                         (p->cfg.flags & GSIM_FLAG_LOG_GLOBAL_EVENTS) != 0, counts))
     return GSIM_ERR_CUDA;
   if (!counts[0]) return GSIM_OK;
@@ -1840,15 +1878,17 @@ static bool long_windows_on() {
 
 // After single ticks: has the pool been quiet long enough, and how far is the horizon?
 static int try_quiet(gsim_pool* p) {
-  GsBackend* be = p->be;
+  GsBackend* be = dev(p);
   const GsGlobals& g = p->g;
   const uint32_t depth = g.ring_mask + 1u;
   uint32_t* qs = p->d.qstate[p->sharded ? p->rank : 0u];
-  if (p->sharded && !be->xbar_host(p->xb)) return GSIM_ERR_CUDA;  // every rank's last tick has published
-  uint32_t la = 0;
-  if (!be->d2h(&la, qs + GS_Q_LAST_ACTIVE, 4)) return GSIM_ERR_CUDA;
-  // ... and nobody runs on (and writes this rank's copy from its next tick) before everybody has read
-  if (p->sharded && !be->xbar_host(p->xb)) return GSIM_ERR_CUDA;
+  uint32_t la = p->last_active;  // single GPU: the word run_ticks read back with its own synchronisation
+  if (p->sharded) {
+    if (!be->xbar_host(p->xb)) return GSIM_ERR_CUDA;  // every rank's last tick has published
+    if (!be->d2h(&la, qs + GS_Q_LAST_ACTIVE, 4)) return GSIM_ERR_CUDA;
+    // ... and nobody runs on (and writes this rank's copy from its next tick) before everybody has read
+    if (!be->xbar_host(p->xb)) return GSIM_ERR_CUDA;
+  }
   if (p->dirty_tick + 1u > la) la = p->dirty_tick + 1u;  // a host write at tick T counts like mail at T
   // every arrival slot has been scanned empty once and nobody posted meanwhile: `depth` quiet ticks
   if (p->now < la + depth) {
@@ -1861,35 +1901,44 @@ static int try_quiet(gsim_pool* p) {
     return GSIM_OK;
   }
   p->quiet_fails = 0;
-  const uint32_t never = GS_NEVER;
-  if (!be->h2d(qs + GS_Q_HORIZON, &never, 4)) return GSIM_ERR_CUDA;
-  if (p->sharded && !be->xbar_host(p->xb)) return GSIM_ERR_CUDA;
-  uint32_t first = 0, count = g.n;
-  if (p->sharded) {
-    first = p->rank * (uint32_t)p->rows_per_rank < g.n ? p->rank * (uint32_t)p->rows_per_rank : g.n;
-    count = first + (uint32_t)p->rows_per_rank < g.n ? (uint32_t)p->rows_per_rank : g.n - first;
-  }
-  if (!be->quiet_scan(p->d, p->g_dev, g, p->now, first, count)) return GSIM_ERR_CUDA;
-  if (p->sharded && !be->xbar_host(p->xb)) return GSIM_ERR_CUDA;
-  p->sched_counts[3]++;
+  // No probe in flight, and can one fail at all?  Not if every member the cluster lists as alive or
+  // suspect is actually running, no packet is lost and no link is slower than ProbeTimeout: then the
+  // horizon cannot move and one launch may run many ProbeIntervals (the controller counts, every
+  // rank adopts the answer).
+  bool links_ok = true;  // every round trip of the latency matrix fits ProbeTimeout
+  for (uint32_t a = 0; a < g.n_dcs && links_ok; ++a)
+    for (uint32_t b = 0; b < g.n_dcs; ++b)
+      if ((uint32_t)g.lat[a * GS_MAX_DCS + b] + g.lat[b * GS_MAX_DCS + a] > g.T) links_ok = false;
+  const bool can_long = g.loss_thr == 0u && p->n_impaired == 0u && links_ok;
   uint32_t hz = 0;
-  if (!be->d2h(&hz, qs + GS_Q_HORIZON, 4)) return GSIM_ERR_CUDA;
-  if (p->sharded && !be->xbar_host(p->xb)) return GSIM_ERR_CUDA;  // (same: read before anybody moves on)
+  if (!p->sharded) {
+    // horizon reset, scan and readback in one round trip, with the counts a long window needs
+    counts_invalidate(p);  // (ticks have run since the last count)
+    if (!upload_globals(p)) return GSIM_ERR_CUDA;
+    if (!be->quiet_probe(p->d, p->g_dev, g, p->now, &hz, can_long ? &p->rc : nullptr)) return GSIM_ERR_CUDA;
+    p->counts_stale = !can_long;
+  } else {
+    const uint32_t never = GS_NEVER;
+    if (!be->h2d(qs + GS_Q_HORIZON, &never, 4)) return GSIM_ERR_CUDA;
+    if (!be->xbar_host(p->xb)) return GSIM_ERR_CUDA;
+    uint32_t first, count;
+    shard_rows(p, &first, &count);
+    if (!be->quiet_scan(p->d, p->g_dev, g, p->now, first, count)) return GSIM_ERR_CUDA;
+    if (!be->xbar_host(p->xb)) return GSIM_ERR_CUDA;
+    if (!be->d2h(&hz, qs + GS_Q_HORIZON, 4)) return GSIM_ERR_CUDA;
+    if (!be->xbar_host(p->xb)) return GSIM_ERR_CUDA;  // (same: read before anybody moves on)
+  }
+  p->sched_counts[3]++;
   if (hz >= p->now + g.P / 2u + 1u) {
     p->quiet = true;
-    // No probe in flight, and can one fail at all?  Not if every member the cluster lists as alive or
-    // suspect is actually running, no packet is lost and no link is slower than ProbeTimeout: then the
-    // horizon cannot move and one launch may run many ProbeIntervals (the controller counts, every
-    // rank adopts the answer).
     uint32_t ok_long = 0;
-    bool links_ok = true;  // every round trip of the latency matrix fits ProbeTimeout
-    for (uint32_t a = 0; a < g.n_dcs && links_ok; ++a)
-      for (uint32_t b = 0; b < g.n_dcs; ++b)
-        if ((uint32_t)g.lat[a * GS_MAX_DCS + b] + g.lat[b * GS_MAX_DCS + a] > g.T) links_ok = false;
-    if (hz == GS_NEVER && g.loss_thr == 0u && p->n_impaired == 0u && links_ok) {
-      counts_invalidate(p);  // (ticks have run since the last count)
-      int rc = collective_recount(p);
-      if (rc) return rc;
+    if (hz == GS_NEVER && can_long) {
+      int rc = GSIM_OK;
+      if (p->sharded) {
+        counts_invalidate(p);  // (ticks have run since the last count)
+        rc = collective_recount(p);
+        if (rc) return rc;
+      }
       rc = controller_call(p, &ok_long, sizeof(ok_long), [&]() -> int {
         if (!do_recount(p)) return GSIM_ERR_CUDA;
         ok_long = p->rc.unreachable_live == 0u ? 1u : 0u;
@@ -1915,7 +1964,7 @@ static int try_quiet(gsim_pool* p) {
 
 // `chunk` ticks, as quiet windows where the pool allows it and as single ticks where it does not.
 static int advance_ticks(gsim_pool* p, uint32_t chunk, bool use_graph) {
-  GsBackend* be = p->be;
+  GsBackend* be = dev(p);
   const GsXbar* xb = p->sharded ? &p->xb : nullptr;
   uint32_t left = chunk;
   const bool can_window = windows_possible(p);
@@ -1954,7 +2003,7 @@ static int advance_ticks(gsim_pool* p, uint32_t chunk, bool use_graph) {
     if (can_window && c > 16u) c = 16u;  // look for quietness every few ticks
     if (can_window && p->retry_at > p->now && p->retry_at - p->now < c) c = p->retry_at - p->now;
     double tms = 0;
-    if (!be->run_ticks(p->d, p->g_dev, p->g, p->now, c, use_graph, &tms, &p->last_launches, xb))
+    if (!be->run_ticks_read(p->d, p->g_dev, p->g, p->now, c, use_graph, &tms, &p->last_launches, xb, &p->last_active))
       return GSIM_ERR_CUDA;
     p->last_ms += tms;
     p->sched_counts[5] += (uint64_t)(tms * 1e6);
@@ -2046,7 +2095,7 @@ extern "C" int gsim_run_until(gsim_pool* p, int predicate, uint32_t arg, uint32_
       if (!peek(p, p->d.conv_tick, arg, &result)) return fail(p, GSIM_ERR_CUDA, "peek");
     } else if (predicate == GSIM_PRED_ALL_RUMORS_CONVERGED) {
       uint32_t ct[32];
-      if (!p->be->d2h(ct, p->d.conv_tick, sizeof(ct))) return fail(p, GSIM_ERR_CUDA, "d2h");
+      if (!dev(p)->d2h(ct, p->d.conv_tick, sizeof(ct))) return fail(p, GSIM_ERR_CUDA, "d2h");
       uint32_t mx = 0;
       bool all = true;
       for (uint32_t r = 0; r < GS_MAX_RUMORS; ++r)
@@ -2091,9 +2140,9 @@ static bool host_knows(const GsGlobals& g, uint32_t i, uint32_t c, uint32_t kc, 
 // Pinned staging for bulk reads (Members() pulls one key per member): grown on demand, freed with the pool.
 static uint32_t* host_stage(gsim_pool* p, size_t words) {
   if (words > p->stage_words) {
-    if (p->stage) p->be->host_free(p->stage);
+    if (p->stage) dev(p)->host_free(p->stage);
     p->stage_words = 0;
-    p->stage = static_cast<uint32_t*>(p->be->host_alloc(words * 4u));
+    p->stage = static_cast<uint32_t*>(dev(p)->host_alloc(words * 4u));
     if (p->stage) p->stage_words = words;
   }
   return p->stage;
@@ -2104,7 +2153,7 @@ static int members_locked(gsim_pool* p, uint32_t observer, gsim_member* out, siz
   if (observer >= g.n) return GSIM_ERR_NOT_FOUND;
   uint32_t* keys = host_stage(p, g.n);
   uint32_t heard, meta;
-  if (!keys || !p->be->d2h(keys, p->d.key[p->now & 1u], (size_t)g.n * 4) ||
+  if (!keys || !dev(p)->d2h(keys, p->d.key[p->now & 1u], (size_t)g.n * 4) ||
       !peek(p, p->d.heard, observer, &heard) || !peek(p, p->d.meta, observer, &meta))
     return GSIM_ERR_CUDA;
   // on a CSR peer graph a member's list is itself plus its row
@@ -2201,10 +2250,10 @@ extern "C" int gsim_poll_events(gsim_pool* p, gsim_event* out, size_t cap, size_
   std::lock_guard<std::mutex> lk(p->mu);
   GS_CONTROLLER_ONLY(p);
   uint32_t cur[2];
-  if (!p->be->d2h(cur, p->d.evlog_cursor, 8)) return fail(p, GSIM_ERR_CUDA, "d2h");
+  if (!dev(p)->d2h(cur, p->d.evlog_cursor, 8)) return fail(p, GSIM_ERR_CUDA, "d2h");
   uint32_t have = cur[0] < p->g.evlog_cap ? cur[0] : p->g.evlog_cap;
   std::vector<GsEventRec> ev(have);
-  if (have && !p->be->d2h(ev.data(), p->d.evlog, (size_t)have * sizeof(GsEventRec)))
+  if (have && !dev(p)->d2h(ev.data(), p->d.evlog, (size_t)have * sizeof(GsEventRec)))
     return fail(p, GSIM_ERR_CUDA, "d2h");
   // the device appends in scheduling order; canonical order is (tick, type, subject, observer)
   std::sort(ev.begin(), ev.end(), [](const GsEventRec& a, const GsEventRec& b) {
@@ -2225,11 +2274,11 @@ extern "C" int gsim_poll_events(gsim_pool* p, gsim_event* out, size_t cap, size_
   *n = take;
   // keep what did not fit
   uint32_t rest = have - (uint32_t)take;
-  if (rest && !p->be->h2d(p->d.evlog, ev.data() + take, (size_t)rest * sizeof(GsEventRec)))
+  if (rest && !dev(p)->h2d(p->d.evlog, ev.data() + take, (size_t)rest * sizeof(GsEventRec)))
     return fail(p, GSIM_ERR_CUDA, "h2d");
   p->events_dropped += cur[1];
   uint32_t reset[2] = {rest, 0};
-  if (!p->be->h2d(p->d.evlog_cursor, reset, 8)) return fail(p, GSIM_ERR_CUDA, "h2d");
+  if (!dev(p)->h2d(p->d.evlog_cursor, reset, 8)) return fail(p, GSIM_ERR_CUDA, "h2d");
   return GSIM_OK;
 }
 
@@ -2295,12 +2344,12 @@ extern "C" int gsim_stats_get(gsim_pool* p, gsim_stats* out) {
   memset(out, 0, sizeof(*out));
   if (!do_recount(p)) return fail(p, GSIM_ERR_CUDA, "recount");
   if (!p->sharded) {
-    if (!p->be->d2h(out->counters, p->d.stats, sizeof(out->counters))) return fail(p, GSIM_ERR_CUDA, "d2h");
+    if (!dev(p)->d2h(out->counters, p->d.stats, sizeof(out->counters))) return fail(p, GSIM_ERR_CUDA, "d2h");
   } else {
     // message counters are accumulated per rank (no cross-GPU atomics in the tick): sum the pages
     for (uint32_t r = 0; r < p->world; ++r) {
       uint64_t part[GSIM_STAT_COUNT];
-      if (!p->be->d2h(part, p->pages + (size_t)r * GS_PAGE_BYTES + GS_PG_STATS, sizeof(part)))
+      if (!dev(p)->d2h(part, p->pages + (size_t)r * GS_PAGE_BYTES + GS_PG_STATS, sizeof(part)))
         return fail(p, GSIM_ERR_CUDA, "d2h");
       for (int q = 0; q < GSIM_STAT_COUNT; ++q) out->counters[q] += part[q];
     }
@@ -2323,7 +2372,7 @@ extern "C" int gsim_stats_get(gsim_pool* p, gsim_stats* out) {
   out->probe_timeout_ticks = g.T;
   out->gossip_interval_ticks = g.GI;
   uint32_t cur[2] = {0, 0};
-  p->be->d2h(cur, p->d.evlog_cursor, 8);
+  dev(p)->d2h(cur, p->d.evlog_cursor, 8);
   out->events_dropped = p->events_dropped + cur[1];
   return GSIM_OK;
   });
@@ -2334,7 +2383,7 @@ extern "C" int gsim_state_hash(gsim_pool* p, uint64_t out[4]) {
   std::lock_guard<std::mutex> lk(p->mu);
   return controller_call(p, out, 4 * sizeof(uint64_t), [&]() -> int {
   if (!upload_globals(p)) return fail(p, GSIM_ERR_CUDA, "upload");
-  if (!p->be->state_hash(p->d, p->g_dev, p->g, p->now, out)) return fail(p, GSIM_ERR_CUDA, "hash");
+  if (!dev(p)->state_hash(p->d, p->g_dev, p->g, p->now, out)) return fail(p, GSIM_ERR_CUDA, "hash");
   // pool-wide scalars
   uint64_t h = gs_mix64(0x243F6A8885A308D3ull, p->now);
   h = gs_mix64(h, p->g.n);
@@ -2394,7 +2443,7 @@ extern "C" int gsim_column_read(gsim_pool* p, int column, void* out, size_t cap_
     std::vector<uint8_t> pair(ucap * 2);
     uint8_t* o = reinterpret_cast<uint8_t*>(out);
     for (size_t q = 0; q < GS_MAX_RUMORS / 2; ++q) {
-      if (!p->be->d2h(pair.data(), reinterpret_cast<const uint8_t*>(src) + q * cap * 2, ucap * 2))
+      if (!dev(p)->d2h(pair.data(), reinterpret_cast<const uint8_t*>(src) + q * cap * 2, ucap * 2))
         return fail(p, GSIM_ERR_CUDA, "d2h");
       for (size_t i = 0; i < ucap; ++i) {
         o[(2 * q) * ucap + i] = pair[2 * i];
@@ -2404,7 +2453,7 @@ extern "C" int gsim_column_read(gsim_pool* p, int column, void* out, size_t cap_
     return GSIM_OK;
   }
   for (size_t q = 0; q < planes; ++q)
-    if (!p->be->d2h(reinterpret_cast<uint8_t*>(out) + q * ucap * elem,
+    if (!dev(p)->d2h(reinterpret_cast<uint8_t*>(out) + q * ucap * elem,
                     reinterpret_cast<const uint8_t*>(src) + q * cap * elem, ucap * elem))
       return fail(p, GSIM_ERR_CUDA, "d2h");
   if (column == GSIM_COL_META) {
@@ -2553,7 +2602,7 @@ extern "C" int gsim_snapshot(gsim_pool* p, void* out, size_t cap_bytes, size_t* 
     const size_t pb = c.bytes / c.planes;
     for (uint32_t q = 0; q < c.planes; ++q) {
       uint8_t* raw = w + 4;
-      if (!p->be->d2h(raw, reinterpret_cast<uint8_t*>(c.ptr) + (size_t)q * pb, pb)) return fail(p, GSIM_ERR_CUDA, "d2h");
+      if (!dev(p)->d2h(raw, reinterpret_cast<uint8_t*>(c.ptr) + (size_t)q * pb, pb)) return fail(p, GSIM_ERR_CUDA, "d2h");
       // one repeated word?  (buf[0..n-4) == buf[4..n) iff all 32-bit words are equal)
       const bool uniform = c.may_fill && pb >= 8 && memcmp(raw, raw + 4, pb - 4) == 0;
       const uint32_t tag = uniform ? 1u : 0u;
@@ -2611,11 +2660,11 @@ extern "C" int gsim_restore(gsim_pool* p, const void* blob, size_t n_bytes) {
         memcpy(&word, r + 4, 4);
         uint8_t* dst = reinterpret_cast<uint8_t*>(c.ptr) + (size_t)q * pb;
         if (tag == 1u) {
-          if (!p->be->fill32(reinterpret_cast<uint32_t*>(dst), word, pb / 4)) return fail(p, GSIM_ERR_CUDA, "fill");
+          if (!dev(p)->fill32(reinterpret_cast<uint32_t*>(dst), word, pb / 4)) return fail(p, GSIM_ERR_CUDA, "fill");
           r += 8;
         } else if (tag == 0u) {
           if ((size_t)(end - r) < 4 + pb) return fail(p, GSIM_ERR_INVALID, "truncated");
-          if (!p->be->h2d_async(dst, r + 4, pb)) return fail(p, GSIM_ERR_CUDA, "h2d");
+          if (!dev(p)->h2d_async(dst, r + 4, pb)) return fail(p, GSIM_ERR_CUDA, "h2d");
           r += 4 + pb;
         } else {
           return fail(p, GSIM_ERR_INVALID, "corrupt snapshot");
@@ -2625,26 +2674,26 @@ extern "C" int gsim_restore(gsim_pool* p, const void* blob, size_t n_bytes) {
     }
     if ((size_t)(end - r) < 4 + c.bytes) return fail(p, GSIM_ERR_INVALID, "truncated");
     r += 4;  // tag 0 (these columns are always stored raw)
-    if (!p->be->h2d_async(c.ptr, r, c.bytes)) return fail(p, GSIM_ERR_CUDA, "h2d");
+    if (!dev(p)->h2d_async(c.ptr, r, c.bytes)) return fail(p, GSIM_ERR_CUDA, "h2d");
     if (p->sharded && (c.ptr == p->d.key[0] || c.ptr == p->d.key[1])) {
       // the key column is replicated per rank: restore every replica
       uint32_t* rep0 = c.ptr == p->d.key[0] ? p->d.key_rep[0] : p->d.key_rep[1];
       for (uint32_t q = 0; q < p->world; ++q)
-        if (!p->be->h2d_async(rep0 + (size_t)q * p->g.key_stride, r, c.bytes)) return fail(p, GSIM_ERR_CUDA, "h2d");
+        if (!dev(p)->h2d_async(rep0 + (size_t)q * p->g.key_stride, r, c.bytes)) return fail(p, GSIM_ERR_CUDA, "h2d");
     }
     if (p->sharded && c.ptr == (void*)p->d.stats) {
       // counters restore into rank 0's page; the other ranks' partial sums restart at zero
       std::vector<uint8_t> zeros(c.bytes, 0);
       for (uint32_t q = 1; q < p->world; ++q)
-        if (!p->be->h2d(p->pages + (size_t)q * GS_PAGE_BYTES + GS_PG_STATS, zeros.data(), c.bytes)) return fail(p, GSIM_ERR_CUDA, "h2d");
+        if (!dev(p)->h2d(p->pages + (size_t)q * GS_PAGE_BYTES + GS_PG_STATS, zeros.data(), c.bytes)) return fail(p, GSIM_ERR_CUDA, "h2d");
     }
     r += c.bytes;
   }
   // a blob without impairment columns restores a pool nobody in it is impaired
   if (!blob_impaired && p->imp_loss &&
-      (!p->be->fill32(p->imp_loss, 0, p->g.cap) || !p->be->fill8(p->imp_delay, 0, p->g.cap)))
+      (!dev(p)->fill32(p->imp_loss, 0, p->g.cap) || !dev(p)->fill8(p->imp_delay, 0, p->g.cap)))
     return fail(p, GSIM_ERR_CUDA, "fill");
-  if (!p->be->sync()) return fail(p, GSIM_ERR_CUDA, "sync");  // every plane has left the caller's blob
+  if (!dev(p)->sync()) return fail(p, GSIM_ERR_CUDA, "sync");  // every plane has left the caller's blob
   {
     // topology fields stay the live pool's (they were checked equal above, except the rank, which is
     // this process's own on a sharded pool)
@@ -2663,10 +2712,10 @@ extern "C" int gsim_restore(gsim_pool* p, const void* blob, size_t n_bytes) {
   if (!impair_recount(p)) return fail(p, GSIM_ERR_CUDA, "d2h");
   if (!poke(p, p->d.tick_base, 0, p->now) || !reset_tick_flags(p) || !reset_qstate(p)) return fail(p, GSIM_ERR_CUDA, "poke");
   uint32_t zero2[2] = {0, 0};
-  if (!p->be->h2d(p->d.evlog_cursor, zero2, 8)) return fail(p, GSIM_ERR_CUDA, "h2d");
+  if (!dev(p)->h2d(p->d.evlog_cursor, zero2, 8)) return fail(p, GSIM_ERR_CUDA, "h2d");
   return GSIM_OK;
   });
-  p->be->sync();  // whatever happened, no copy out of the caller's blob is still in flight
+  dev(p)->sync();  // whatever happened, no copy out of the caller's blob is still in flight
   return rc_all;
 }
 
@@ -2678,7 +2727,7 @@ extern "C" int gsim_last_step_timing(gsim_pool* p, double* kernel_ms, uint64_t* 
   return GSIM_OK;
 }
 
-extern "C" uint64_t gsim_launch_count(gsim_pool* p) { return p && p->be ? p->be->total_launches() : 0; }
+extern "C" uint64_t gsim_launch_count(gsim_pool* p) { return p && p->be ? dev(p)->total_launches() : 0; }
 
 // ---- wire formats (include/gsim.h; encoders in gs_wire.h) ---------------------------------------
 static size_t zlen(const char* s) { return s ? strlen(s) : 0; }

@@ -24,6 +24,52 @@ struct GsRecount {
                               // still lists as alive or suspect: the targets an unanswered probe can hit
 };
 
+// ---- device write batches -------------------------------------------------------------------
+// The host side of an operation (a new member, a join, a retired rumor) is a few dozen small writes,
+// several of them read-modify-writes of a word the host does not keep.  They are queued as an ordered
+// list and applied on the device in that order by one thread, after everything the pool enqueued
+// before and before everything it enqueues after: no host round trip per word.
+enum : uint32_t {
+  GS_WR_STORE32 = 0,  // *a = v
+  GS_WR_STORE8 = 1,   // byte *a = v
+  GS_WR_OR32 = 2,     // *a |= v
+  GS_WR_AND32 = 3,    // *a &= v
+  GS_WR_KST = 4,      // status byte a (gs_kst_code): nibble v (0 = low, key[0]; 1 = high, key[1]) := code of key word b
+  GS_WR_HEARD = 5,    // heard_cnt[r] at a += v; if that makes it w (up_count) and conv_tick[r] at b is empty, it := x (now)
+};
+struct GsWriteOp {
+  uint64_t a, b;  // device addresses
+  uint32_t op, v, w, x;
+};
+#define GS_WB_MAX 120u  // ops per launch: the batch travels as one kernel parameter (< 4 KB)
+struct GsWriteBatch {
+  uint32_t n, pad;
+  GsWriteOp op[GS_WB_MAX];
+};
+
+GS_HD void gs_apply_write(const GsWriteOp& o) {
+  uint32_t* a = reinterpret_cast<uint32_t*>(o.a);
+  switch (o.op) {
+    case GS_WR_STORE32: *a = o.v; break;
+    case GS_WR_STORE8: *reinterpret_cast<uint8_t*>(o.a) = (uint8_t)o.v; break;
+    case GS_WR_OR32: *a |= o.v; break;
+    case GS_WR_AND32: *a &= o.v; break;
+    case GS_WR_KST: {
+      uint8_t* s = reinterpret_cast<uint8_t*>(o.a);
+      const uint32_t code = gs_kst_code(*reinterpret_cast<const uint32_t*>(o.b));
+      *s = (uint8_t)(o.v ? ((*s & 0x0Fu) | (code << 4)) : ((*s & 0xF0u) | code));
+      break;
+    }
+    case GS_WR_HEARD: {
+      const uint32_t c = *a + o.v;
+      *a = c;
+      uint32_t* conv = reinterpret_cast<uint32_t*>(o.b);
+      if (c == o.w && *conv == GS_EMPTY32) *conv = o.x;
+      break;
+    }
+  }
+}
+
 class GsBackend {
  public:
   virtual ~GsBackend() {}
@@ -32,11 +78,32 @@ class GsBackend {
   virtual void release(void* p) = 0;
   virtual bool h2d(void* dst, const void* src, size_t bytes) = 0;
   virtual bool d2h(void* dst, const void* src, size_t bytes) = 0;
-  // A few bytes host -> device, ordered on the pool's stream but NOT waited for: the source may be reused
-  // as soon as the call returns (the driver stages small pageable copies before returning), everything
-  // the pool launches or reads later comes after it.  The host side of Join / UserEvent is dozens of
-  // single-word writes; waiting for each one was most of its cost.
+  // A few KB at most host -> device, ordered on the pool's stream but NOT waited for: the source may be
+  // reused as soon as the call returns (the driver stages small pageable copies before returning),
+  // everything the pool launches or reads later comes after it.  Used for the globals upload.
   virtual bool h2d_word(void* dst, const void* src, size_t bytes) { return h2d(dst, src, bytes); }
+  // The ops of `b` in order, on the pool's stream (see GsWriteBatch).  The CUDA backend applies them in
+  // one launch that is not waited for and ends in a system-scope fence, so peers of a sharded pool see
+  // every op once a barrier that comes after it on this stream has let them go on.  Defined here
+  // through the copy primitives every backend has, which is what the host emulation runs.
+  virtual bool write_batch(const GsWriteBatch& b) {
+    for (uint32_t k = 0; k < b.n; ++k) {
+      const GsWriteOp& o = b.op[k];
+      const size_t na = (o.op == GS_WR_STORE8 || o.op == GS_WR_KST) ? 1u : 4u;
+      const bool use_b = o.op == GS_WR_KST || o.op == GS_WR_HEARD;
+      uint32_t a = 0u, bw = 0u;  // host copies of the words the op touches
+      if (!d2h(&a, reinterpret_cast<const void*>(o.a), na)) return false;
+      if (use_b && !d2h(&bw, reinterpret_cast<const void*>(o.b), 4)) return false;
+      const uint32_t b0 = bw;
+      GsWriteOp h = o;
+      h.a = (uint64_t)(uintptr_t)&a;
+      h.b = (uint64_t)(uintptr_t)&bw;
+      gs_apply_write(h);
+      if (!h2d(reinterpret_cast<void*>(o.a), &a, na)) return false;
+      if (bw != b0 && !h2d(reinterpret_cast<void*>(o.b), &bw, 4)) return false;
+    }
+    return true;
+  }
   // Bulk host -> device, enqueued only: the caller keeps `src` alive and calls sync() before it returns
   // (gsim_restore streams its planes back to back and waits once).
   // host staging memory for bulk copies (page-locked where that makes the copy a plain DMA)
@@ -46,9 +113,15 @@ class GsBackend {
   // The per-member words the host side of a state exchange needs, in one round trip:
   // out = {key[0], key[1], meta, heard, queued, ltime_member, ltime_event, event_min}
   virtual bool row_read(const GsDev& d, uint32_t i, uint32_t out[8]) = 0;
+  // ... for `n` members, out[8 * x ..] = the words of ids[x] (the CUDA backend: one round trip per 64 rows)
+  virtual bool rows_read(const GsDev& d, const uint32_t* ids, uint32_t n, uint32_t* out) {
+    for (uint32_t x = 0; x < n; ++x)
+      if (!row_read(d, ids[x], out + 8 * (size_t)x)) return false;
+    return true;
+  }
   virtual bool fill32(uint32_t* dst, uint32_t value, size_t count) = 0;
   virtual bool fill8(uint8_t* dst, uint8_t value, size_t count) = 0;
-  // rows [first, first+count): converged members, inc=1, clocks=1, phases from Philox
+  // rows [first, first+count): converged members, inc=1, clocks=1, phases from Philox (not waited for)
   virtual bool init_rows(const GsDev& d, const GsGlobals* g_dev, const GsGlobals& g, uint32_t first,
                          uint32_t count, uint32_t now) = 0;
   // advance `nticks` ticks starting at tick t0 (tick_base on the device == t0 on entry and
@@ -56,6 +129,14 @@ class GsBackend {
   virtual bool run_ticks(const GsDev& d, const GsGlobals* g_dev, const GsGlobals& g, uint32_t t0,
                          uint32_t nticks, bool use_graph, double* kernel_ms, uint64_t* launches,
                          const GsXbar* xbar = nullptr) = 0;
+  // run_ticks, then *last_active = this rank's GS_Q_LAST_ACTIVE.  The CUDA backend reads it back with
+  // the launches' own synchronisation; by default it is a readback of its own.
+  virtual bool run_ticks_read(const GsDev& d, const GsGlobals* g_dev, const GsGlobals& g, uint32_t t0, uint32_t nticks,
+                              bool use_graph, double* kernel_ms, uint64_t* launches, const GsXbar* xbar,
+                              uint32_t* last_active) {
+    return run_ticks(d, g_dev, g, t0, nticks, use_graph, kernel_ms, launches, xbar) &&
+           d2h(last_active, d.qstate[g.rank] + GS_Q_LAST_ACTIVE, 4);
+  }
   // Quiet windows (DESIGN.md §4.2): advance up to `nticks` ticks starting at t0 as a chain of launches
   // of <= ProbeInterval ticks each, on a pool whose mailboxes are known to be empty.  The chain stops at
   // the horizon (GS_Q_HORIZON); *ticks_done = how far it got (tick_base == t0 + *ticks_done on exit).
@@ -68,6 +149,15 @@ class GsBackend {
   // [first, first+count) can produce
   virtual bool quiet_scan(const GsDev& d, const GsGlobals* g_dev, const GsGlobals& g, uint32_t now, uint32_t first,
                           uint32_t count) = 0;
+  // Single-GPU pools: GS_Q_HORIZON := GS_NEVER, quiet_scan over every member, *horizon = the result, and
+  // (counts != nullptr) recount over every member into *counts.  The CUDA backend makes it one submission
+  // with one readback; by default it is the primitives one after the other.
+  virtual bool quiet_probe(const GsDev& d, const GsGlobals* g_dev, const GsGlobals& g, uint32_t now,
+                           uint32_t* horizon, GsRecount* counts) {
+    const uint32_t never = GS_NEVER;
+    return h2d(d.qstate[0] + GS_Q_HORIZON, &never, 4) && quiet_scan(d, g_dev, g, now, 0u, g.n) &&
+           d2h(horizon, d.qstate[0] + GS_Q_HORIZON, 4) && (!counts || recount(d, g_dev, g, now, 0u, g.n, counts));
+  }
   // ---- sharded (multi-GPU) pools, see gs_vmm.h; unsupported by default ------------------------
   virtual bool shard_begin(uint32_t, uint32_t) { return false; }
   virtual size_t shard_granularity() { return 0; }
@@ -108,7 +198,7 @@ class GsBackend {
   virtual bool reap_rows(const GsDev& d, const GsGlobals* g_dev, const GsGlobals& g, uint32_t now,
                          uint32_t reconnect_ticks, uint32_t tombstone_ticks, bool log_events,
                          uint32_t counts[2]) = 0;
-  // clear rumor bits outside `keep` in the heard / queued / mailbox columns (slot retirement)
+  // clear rumor bits outside `keep` in the heard / queued / mailbox columns (slot retirement; not waited for)
   virtual bool and_columns(const GsDev& d, const GsGlobals& g, uint32_t keep, uint32_t first, uint32_t count) = 0;
   virtual bool sync() = 0;
   virtual const char* last_error() const = 0;

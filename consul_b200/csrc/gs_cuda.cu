@@ -1027,10 +1027,26 @@ static cudaError_t gs_launch_window(uint32_t blocks, cudaStream_t stream, const 
                  : cudaLaunchKernelEx(&cfg, gs_window_kernel<false, false>, d, g_dev, k_off, n_ticks, mode);
 }
 
-__global__ void gs_row_read_kernel(GsDev d, uint32_t i, uint32_t* out) {
+#define GS_ROWS_MAX 64u  // rows one gs_rows_read_kernel launch gathers (8 words each: 2 KB of scratch)
+struct GsRowIds {
+  uint32_t n;
+  uint32_t id[GS_ROWS_MAX];
+};
+__global__ void gs_rows_read_kernel(GsDev d, GsRowIds r, uint32_t* out) {
   const uint32_t* col[8] = {d.key[0], d.key[1], d.meta, d.heard, d.queued, d.ltime_member, d.ltime_event, d.event_min};
-  if (threadIdx.x < 8u) out[threadIdx.x] = col[threadIdx.x][i];
+  const uint32_t t = threadIdx.x;
+  if (t < r.n * 8u) out[t] = col[t & 7u][r.id[t >> 3]];
 }
+
+// A host operation's small writes (GsWriteBatch), in order; the fence makes them visible to the other
+// GPUs of a sharded pool before anything this stream runs later (their barrier) can let those go on.
+__global__ void gs_write_batch_kernel(const __grid_constant__ GsWriteBatch b) {
+  for (uint32_t k = 0; k < b.n; ++k) gs_apply_write(b.op[k]);
+  __threadfence_system();
+}
+
+// The quiet probe's horizon, next to its counts in scratch: one readback for both
+__global__ void gs_copy_word_kernel(uint32_t* dst, const uint32_t* src) { *dst = *src; }
 
 __global__ void __launch_bounds__(GS_BLOCK) gs_fill32_kernel(uint32_t* dst, uint32_t value, size_t count) {
   for (size_t x = (size_t)blockIdx.x * GS_BLOCK + threadIdx.x; x < count; x += (size_t)gridDim.x * GS_BLOCK)
@@ -1109,20 +1125,34 @@ class CudaBackend : public GsBackend {
   }
   void host_free(void* q) override { cudaFreeHost(q); }
   bool h2d_word(void* dst, const void* src, size_t bytes) override {
-    if (bytes > 64) return h2d(dst, src, bytes);
+    if (bytes > 16384) return h2d(dst, src, bytes);
     cudaSetDevice(dev_);
     return ok(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, stream_), "h2d");
+  }
+  bool write_batch(const GsWriteBatch& b) override {
+    if (!b.n) return true;
+    cudaSetDevice(dev_);
+    gs_write_batch_kernel<<<1, 1, 0, stream_>>>(b);
+    ++launches_;
+    return ok(cudaGetLastError(), "write batch launch");
   }
   bool h2d_async(void* dst, const void* src, size_t bytes) override {
     cudaSetDevice(dev_);
     return ok(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, stream_), "h2d");
   }
-  bool row_read(const GsDev& d, uint32_t i, uint32_t out[8]) override {
+  bool row_read(const GsDev& d, uint32_t i, uint32_t out[8]) override { return rows_read(d, &i, 1u, out); }
+  bool rows_read(const GsDev& d, const uint32_t* ids, uint32_t n, uint32_t* out) override {
     cudaSetDevice(dev_);
     uint32_t* w = reinterpret_cast<uint32_t*>(scratch_) + 256;  // (the first KB of scratch belongs to the counters)
-    gs_row_read_kernel<<<1, 32, 0, stream_>>>(d, i, w);
-    ++launches_;
-    return ok(cudaGetLastError(), "row read launch") && d2h(out, w, 32);
+    for (uint32_t x0 = 0; x0 < n; x0 += GS_ROWS_MAX) {
+      GsRowIds r;
+      r.n = n - x0 < GS_ROWS_MAX ? n - x0 : GS_ROWS_MAX;
+      memcpy(r.id, ids + x0, r.n * 4);
+      gs_rows_read_kernel<<<1, GS_ROWS_MAX * 8, 0, stream_>>>(d, r, w);
+      ++launches_;
+      if (!ok(cudaGetLastError(), "rows read launch") || !d2h(out + (size_t)x0 * 8, w, (size_t)r.n * 32)) return false;
+    }
+    return true;
   }
   bool fill32(uint32_t* dst, uint32_t value, size_t count) override {
     cudaSetDevice(dev_);
@@ -1141,19 +1171,25 @@ class CudaBackend : public GsBackend {
     gs_init_kernel<<<(count + GS_BLOCK - 1) / GS_BLOCK, GS_BLOCK, 0, stream_>>>(d, g_dev, first,
                                                                                 count, now);
     ++launches_;
-    return ok(cudaGetLastError(), "init launch") && ok(cudaStreamSynchronize(stream_), "init");
+    return ok(cudaGetLastError(), "init launch");
   }
   bool run_ticks(const GsDev& d, const GsGlobals* g_dev, const GsGlobals& g, uint32_t t0,
                  uint32_t nticks, bool use_graph, double* kernel_ms, uint64_t* launches,
                  const GsXbar* xbar) override {
+    uint32_t last_active = 0;
+    return run_ticks_read(d, g_dev, g, t0, nticks, use_graph, kernel_ms, launches, xbar, &last_active);
+  }
+  bool run_ticks_read(const GsDev& d, const GsGlobals* g_dev, const GsGlobals& g, uint32_t t0, uint32_t nticks,
+                      bool use_graph, double* kernel_ms, uint64_t* launches, const GsXbar* xbar,
+                      uint32_t* last_active) override {
     (void)t0;
     if (!nticks || !g.n) {
       if (nticks) {  // no members: just advance time
         gs_advance_kernel<<<1, 1, 0, stream_>>>(d.tick_base, nticks, nullptr);
         ++launches_;
-        return ok(cudaGetLastError(), "advance") && ok(cudaStreamSynchronize(stream_), "advance");
+        return ok(cudaGetLastError(), "advance") && d2h(last_active, d.qstate[g.rank] + GS_Q_LAST_ACTIVE, 4);
       }
-      return true;
+      return d2h(last_active, d.qstate[g.rank] + GS_Q_LAST_ACTIVE, 4);
     }
     cudaSetDevice(dev_);
     // performance variant: keep the status replica (1 byte per member, gathered at random by every
@@ -1205,11 +1241,14 @@ class CudaBackend : public GsBackend {
     }
     if (!ok(cudaEventRecord(ev1_, stream_), "event")) return false;
     // the word a kernel raises when one of its internal invariants breaks (a bulk copy that never
-    // completed): read back with the synchronisation that happens anyway, so that it fails loudly
-    uint32_t violation = 0;
-    if (!ok(cudaMemcpyAsync(&violation, d.qstate[g.rank] + GS_Q_VIOLATION, 4, cudaMemcpyDeviceToHost, stream_), "tick d2h"))
+    // completed): read back with the synchronisation that happens anyway, so that it fails loudly;
+    // the same 16 bytes carry the last active tick the host's quiet detection needs
+    uint32_t qs[GS_Q_WORDS] = {0, 0, 0, 0};
+    if (!ok(cudaMemcpyAsync(qs, d.qstate[g.rank], sizeof(qs), cudaMemcpyDeviceToHost, stream_), "tick d2h"))
       return false;
     if (!ok(cudaStreamSynchronize(stream_), "tick sync")) return false;
+    const uint32_t violation = qs[GS_Q_VIOLATION];
+    *last_active = qs[GS_Q_LAST_ACTIVE];
     float ms = 0.f;
     cudaEventElapsedTime(&ms, ev0_, ev1_);
     if (kernel_ms) *kernel_ms += ms;
@@ -1294,6 +1333,37 @@ class CudaBackend : public GsBackend {
     ++launches_;
     (void)g;
     return ok(cudaGetLastError(), "quiet scan launch") && ok(cudaStreamSynchronize(stream_), "quiet scan");
+  }
+  bool quiet_probe(const GsDev& d, const GsGlobals* g_dev, const GsGlobals& g, uint32_t now, uint32_t* horizon,
+                   GsRecount* counts) override {
+    cudaSetDevice(dev_);
+    // scratch: [0, sizeof(GsRecount)) the counts, then the horizon word
+    GsRecount* dr = reinterpret_cast<GsRecount*>(scratch_);
+    uint32_t* dh = reinterpret_cast<uint32_t*>(dr + 1);
+    uint32_t* qh = d.qstate[0] + GS_Q_HORIZON;
+    if (!ok(cudaMemsetAsync(qh, 0xFF, 4, stream_), "memset")) return false;  // GS_NEVER
+    if (g.n) {
+      uint32_t blocks = (g.n + GS_BLOCK - 1) / GS_BLOCK;
+      if (blocks > sms_ * 8u) blocks = sms_ * 8u;
+      gs_quiet_scan_kernel<<<blocks, GS_BLOCK, 0, stream_>>>(d, g_dev, now, 0u, g.n);
+      ++launches_;
+    }
+    gs_copy_word_kernel<<<1, 1, 0, stream_>>>(dh, qh);
+    ++launches_;
+    if (counts) {
+      if (!ok(cudaMemsetAsync(dr, 0, sizeof(GsRecount), stream_), "memset")) return false;
+      if (g.n) {
+        gs_recount_kernel<<<(g.n + GS_BLOCK - 1) / GS_BLOCK, GS_BLOCK, 0, stream_>>>(d, g_dev, now, 0u, g.n, dr);
+        ++launches_;
+      }
+    }
+    if (!ok(cudaGetLastError(), "quiet probe launch")) return false;
+    uint8_t back[sizeof(GsRecount) + 4];
+    const size_t off = counts ? 0 : sizeof(GsRecount);
+    if (!d2h(back + off, reinterpret_cast<uint8_t*>(scratch_) + off, sizeof(back) - off)) return false;
+    if (counts) memcpy(counts, back, sizeof(GsRecount));
+    memcpy(horizon, back + sizeof(GsRecount), 4);
+    return true;
   }
   bool crash_fraction(const GsDev& d, const GsGlobals* g_dev, const GsGlobals& g, uint32_t thr,
                       uint32_t salt, uint32_t, uint32_t* n_crashed) override {
@@ -1398,7 +1468,7 @@ class CudaBackend : public GsBackend {
     if (count > g.n - first) count = g.n - first;
     gs_and_kernel<<<(count + GS_BLOCK - 1) / GS_BLOCK, GS_BLOCK, 0, stream_>>>(d, first, count, keep);
     ++launches_;
-    return ok(cudaGetLastError(), "and launch") && ok(cudaStreamSynchronize(stream_), "and");
+    return ok(cudaGetLastError(), "and launch");
   }
   bool sync() override {
     cudaSetDevice(dev_);

@@ -1,5 +1,6 @@
 """Where the end-to-end step of bench.py goes on one GPU: wall time of each C-ABI call (dev tool).
-restore (snapshot blob in pinned host memory) -> member_add -> join -> step(2048) -> Members() -> stats."""
+restore (snapshot blob in pinned host memory) -> member_add -> join -> step(2048) -> Members() -> stats.
+An optional argument names the libgsim build to time (default: the package's)."""
 import ctypes as C
 import json
 import os
@@ -9,11 +10,13 @@ import time
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from consul_b200 import _lib  # noqa: E402
 from consul_b200._lib import GsimMember  # noqa: E402
 from consul_b200.pool import Pool, lan_config  # noqa: E402
 
+lib = _lib.load(sys.argv[1]) if len(sys.argv) > 1 else _lib.lib()
 n = 1_000_000
-p = Pool(lan_config(capacity=n + 4096, n_initial=n, seed=0x5EED0001))
+p = Pool(lan_config(lib, capacity=n + 4096, n_initial=n, seed=0x5EED0001), lib)
 p.step(64)
 blob = p.snapshot()
 pinned = torch.empty(len(blob), dtype=torch.uint8, pin_memory=True)
@@ -35,5 +38,5 @@ for it in range(REP + 2):
     if it >= 2:
         for i, nm in enumerate(names):
             acc[nm] += (ts[i + 1] - ts[i]) * 1e3 / REP
-print(json.dumps({"blob_bytes": len(blob), "members": k.value, "threads": os.environ.get("GSIM_MEMBERS_THREADS"),
+print(json.dumps({"lib": lib._name, "blob_bytes": len(blob), "members": k.value, "threads": os.environ.get("GSIM_MEMBERS_THREADS"),
                   "wall_ms": {a: round(b, 3) for a, b in acc.items()}, "sum_ms": round(sum(acc.values()), 3)}))
