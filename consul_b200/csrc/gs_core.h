@@ -35,6 +35,9 @@
                                  // push-pull requests / clocks in ppreq[][][] / pp_clk[][][]
 #define GS_PPK 4                 // push-pull requests one member serves per tick (smallest ids win)
 #define GS_WAKE_BIT 0x40000000u  // inbox: "process this row" (self-posted or by the host)
+// Invariant: a member with queued != 0 has a wake pending at or before its next gossip tick (the row
+// step posts it for that tick, gs_queue_wake_slot; the host posts it for `now` whenever it queues).
+// A running suspicion timer or a stale key buffer (GS_META_DIRTY) has a wake pending for the next tick.
 #define GS_TILE 128u             // rows per CTA; ticker phases are uniform per tile
 #define GS_NEVER 0xFFFFFFFFu
 #define GS_EMPTY32 0xFFFFFFFFu

@@ -310,8 +310,32 @@ __global__ void __launch_bounds__(GS_BLOCK, GS_MIN_BLOCKS)
   }
   for (uint32_t tile = r_begin; tile < r_end; ++tile) {
     const uint32_t st = tile - r_begin;
-    const uint4 i4 = *reinterpret_cast<const uint4*>(&s_inb[wib][st][lane * 4u]);
+    uint4 i4 = *reinterpret_cast<const uint4*>(&s_inb[wib][st][lane * 4u]);
     const uint4 d4 = *reinterpret_cast<const uint4*>(&s_due[wib][st][lane * 4u]);
+    if (__any_sync(0xFFFFFFFFu, (i4.x | i4.y | i4.z | i4.w) != 0u)) {
+      // Stale mail (gs_mail_is_stale): retired here without a row step — the word is cleared (in global
+      // memory before the __syncthreads that closes the round, so the drain below reads it as empty, and
+      // in the round buffer, so the member stays out of act[] and the fast-path candidates) and counted
+      // as activity.  Not an ACTIVE_ROWS row: it never leaves the scan.
+      const uint32_t m0 = tile * GS_TILE + lane * 4u;
+      const uint4 h4 = __ldcg(reinterpret_cast<const uint4*>(d.heard + m0));
+      uint32_t* const w_cur = d.inbox[t & g.ring_mask] + m0;
+      uint32_t* const w4 = &i4.x;
+      const uint32_t* const h = &h4.x;
+      const uint32_t* const du = &d4.x;
+      bool stale_any = false;
+#pragma unroll
+      for (uint32_t u = 0; u < 4u; ++u) {
+        const bool pp = g.pp_interval != 0u && gs_pp_due(g.pp_interval, g.rot_pp, (m0 + u) / g.phase_group, t);
+        if (w4[u] != 0u && gs_mail_is_stale(g, w4[u], h[u], du[u] == t, pp)) {
+          w_cur[u] = 0u;
+          s_inb[wib][st][lane * 4u + u] = 0u;
+          w4[u] = 0u;
+          stale_any = true;
+        }
+      }
+      if (stale_any) sink.activity();
+    }
     bool mine = (i4.x | i4.y | i4.z | i4.w) != 0u || d4.x == t || d4.y == t || d4.z == t || d4.w == t;
     // periodic push-pull (opt-in): the ticker of this tile's phase group (or, with per-member
     // phases, of one of its members) fires at this tick

@@ -430,8 +430,34 @@ GS_DEV bool gs_tile_probe_gate(const GsGlobals& g, uint32_t tile, uint32_t pslot
   return pp == pslot || pp == pslot_t;
 }
 
+// Arrival slot of the self-wake of a member whose broadcast queue is not empty, posted at tick t: its
+// next gossip tick t + delta (gslot = t % GI, gphase = its gossip phase), where section D can run, instead
+// of t + 1.  On the ticks in between the row has nothing to do for its queue; it is not stepped at all
+// unless other mail or its probe ticker brings it.  Deeper than the ring (GI > ring depth): t + 1.
+//   delta == ring depth writes slot t & ring_mask, the one being consumed at tick t.  That is safe: nobody
+// else posts into it during tick t (every delivery arrives at t + 1 + extra with extra <= depth - 2,
+// which gsim_latency_set and gsim_impair_* validate), the row cleared its own word before it got here,
+// and neither the tick kernel nor the host emulation reads a row's word again after its step.
+GS_DEV uint32_t gs_queue_wake_slot(const GsGlobals& g, uint32_t t, uint32_t gslot, uint32_t gphase) {
+  const uint32_t next = gslot + 1u == g.GI ? 0u : gslot + 1u;  // (t + 1) % GI
+  const uint32_t delta = (gphase >= next ? gphase - next : gphase + g.GI - next) + 1u;
+  return (delta > g.ring_mask + 1u ? t + 1u : t + delta) & g.ring_mask;
+}
+
+// Can mailbox word w (non-zero) of a member be retired at tick t without its row step?  Yes when it
+// carries neither a wake nor auxiliary mail, no probe action or push-pull is due, and every tracked
+// rumor bit in it is one the member has already heard (`heard` = its heard word; bits of retired slots
+// are ignored by the step too).  The step would then only clear the word and mark activity: nothing
+// is fresh, so section A accepts nothing; a suspect or dirty row always has a wake; and a queued row at
+// its gossip tick has one as well (the GS_WAKE_BIT invariant).  heard[i] is written only by row i and by
+// the host between launches, so the answer does not depend on scheduling.
+GS_DEV bool gs_mail_is_stale(const GsGlobals& g, uint32_t w, uint32_t heard, bool due_now, bool pp_now) {
+  return (w & (GS_WAKE_BIT | GS_ACC_BIT)) == 0u && !due_now && !pp_now && (w & g.active_mask & ~heard) == 0u;
+}
+
 // The tick of member i, called only for rows that have mail (inb = inbox[t&1][i] != 0,
-// which includes the self-posted wake bit) or a probe action due (due[i] == t).
+// which includes the self-posted wake bit) or a probe action due (due[i] == t).  Stale mail
+// (gs_mail_is_stale) only clears the word; the tick kernel's scan retires it without calling here.
 // IMPAIRED: the pool has degraded members (GsDev::imp_loss / imp_delay are set).  The other
 // instantiation folds every impairment term away, so a pool without any runs the code it would
 // run without the feature.
@@ -456,10 +482,16 @@ GS_DEV void gs_row_step_body(const GsDev& d, const GsGlobals& g, uint32_t i, uin
   const bool up = truth == GS_TRUTH_UP;
   const bool gossip_slot = up && gslot == gs_meta_gphase(m0);  // gslot = t % GI
   uint32_t queued = up ? d.queued[i] : 0u;
+  // the tracked rumor bits of this arrival tick and, when there are any, what the member has heard
+  const uint32_t rbits = inb & ~(GS_ACC_BIT | GS_WAKE_BIT) & g.active_mask;
+  const uint32_t heard0 = rbits != 0u ? d.heard[i] : 0u;
   if (inb != 0u) d.inbox[icur][i] = 0u;
-  sink.stat(GS_ST_ACTIVE_ROWS, 1);  // scheduling diagnostic: rows that left the 4-byte scan
   // periodic push-pull (opt-in): does this member's push-pull ticker fire now?
   const bool pp_now = up && g.pp_interval != 0u && gs_pp_due(g.pp_interval, g.rot_pp, i / g.phase_group, t);
+  // stale mail: clearing the word was all there was to do (the tick kernel's scan retires such words
+  // before calling the step, so it is not counted as a row that left the scan either)
+  if (inb != 0u && gs_mail_is_stale(g, inb, heard0, due0 == t, pp_now)) return;
+  sink.stat(GS_ST_ACTIVE_ROWS, 1);  // scheduling diagnostic: rows that left the 4-byte scan
 
   // ---- nothing to do this tick (a wake that only keeps the row in the active set) ----
   if ((inb & ~GS_WAKE_BIT) == 0u && gs_key_rank(k0) == GS_RANK_ALIVE && !(up && due0 == t) &&
@@ -468,7 +500,7 @@ GS_DEV void gs_row_step_body(const GsDev& d, const GsGlobals& g, uint32_t i, uin
       gs_key_store(d, g, nxt, i, k0);
       d.meta[i] = m0 & ~GS_META_DIRTY;
     }
-    if (queued != 0u) gs_post(d, g, sink, inxt, i, GS_WAKE_BIT);
+    if (queued != 0u) gs_post(d, g, sink, gs_queue_wake_slot(g, t, gslot, gs_meta_gphase(m0)), i, GS_WAKE_BIT);
     return;
   }
 
@@ -492,9 +524,8 @@ GS_DEV void gs_row_step_body(const GsDev& d, const GsGlobals& g, uint32_t i, uin
         }
       }
     }
-    uint32_t rbits = inb & ~(GS_ACC_BIT | GS_WAKE_BIT) & g.active_mask;
     if (rbits && up) {
-      heard = d.heard[i];
+      heard = heard0;
       uint32_t fresh = rbits & ~heard;
       uint32_t accepted = 0;
       while (fresh) {
@@ -870,9 +901,11 @@ GS_DEV void gs_row_step_body(const GsDev& d, const GsGlobals& g, uint32_t i, uin
   if (m != m0) d.meta[i] = m;
   if (due != due0) d.due[i] = due;
   // stay in the active set while something time-driven is pending: a running suspicion
-  // timer, a stale key buffer, or a non-empty broadcast queue
-  if (gs_key_rank(k) == GS_RANK_SUSPECT || (m & GS_META_DIRTY) || queued != 0u)
+  // timer or a stale key buffer (next tick), a non-empty broadcast queue (next gossip tick)
+  if (gs_key_rank(k) == GS_RANK_SUSPECT || (m & GS_META_DIRTY))
     gs_post(d, g, sink, inxt, i, GS_WAKE_BIT);
+  else if (queued != 0u)
+    gs_post(d, g, sink, gs_queue_wake_slot(g, t, gslot, gs_meta_gphase(m)), i, GS_WAKE_BIT);
 }
 
 template <class Sink>
