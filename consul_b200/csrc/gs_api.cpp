@@ -1876,7 +1876,22 @@ static bool long_windows_on() {
   return !off;
 }
 
-// After single ticks: has the pool been quiet long enough, and how far is the horizon?
+// No probe in flight, and can one fail at all?  Not if every member the cluster lists as alive or
+// suspect is actually running, no packet is lost and no link is slower than ProbeTimeout: then the
+// horizon cannot move and one launch may run many ProbeIntervals (the controller counts, every
+// rank adopts the answer).
+static bool probes_always_answered(const gsim_pool* p) {
+  const GsGlobals& g = p->g;
+  bool links_ok = true;  // every round trip of the latency matrix fits ProbeTimeout
+  for (uint32_t a = 0; a < g.n_dcs && links_ok; ++a)
+    for (uint32_t b = 0; b < g.n_dcs; ++b)
+      if ((uint32_t)g.lat[a * GS_MAX_DCS + b] + g.lat[b * GS_MAX_DCS + a] > g.T) links_ok = false;
+  return g.loss_thr == 0u && p->n_impaired == 0u && links_ok;
+}
+static int quiet_decision(gsim_pool* p, uint32_t hz, bool can_long);
+
+// After single ticks (sharded pools, and pools without CUDA graphs): has the pool been quiet long
+// enough, and how far is the horizon?
 static int try_quiet(gsim_pool* p) {
   GsBackend* be = dev(p);
   const GsGlobals& g = p->g;
@@ -1901,15 +1916,7 @@ static int try_quiet(gsim_pool* p) {
     return GSIM_OK;
   }
   p->quiet_fails = 0;
-  // No probe in flight, and can one fail at all?  Not if every member the cluster lists as alive or
-  // suspect is actually running, no packet is lost and no link is slower than ProbeTimeout: then the
-  // horizon cannot move and one launch may run many ProbeIntervals (the controller counts, every
-  // rank adopts the answer).
-  bool links_ok = true;  // every round trip of the latency matrix fits ProbeTimeout
-  for (uint32_t a = 0; a < g.n_dcs && links_ok; ++a)
-    for (uint32_t b = 0; b < g.n_dcs; ++b)
-      if ((uint32_t)g.lat[a * GS_MAX_DCS + b] + g.lat[b * GS_MAX_DCS + a] > g.T) links_ok = false;
-  const bool can_long = g.loss_thr == 0u && p->n_impaired == 0u && links_ok;
+  const bool can_long = probes_always_answered(p);
   uint32_t hz = 0;
   if (!p->sharded) {
     // horizon reset, scan and readback in one round trip, with the counts a long window needs
@@ -1928,6 +1935,14 @@ static int try_quiet(gsim_pool* p) {
     if (!be->d2h(&hz, qs + GS_Q_HORIZON, 4)) return GSIM_ERR_CUDA;
     if (!be->xbar_host(p->xb)) return GSIM_ERR_CUDA;  // (same: read before anybody moves on)
   }
+  return quiet_decision(p, hz, can_long);
+}
+
+// The pool is quiet at p->now and the horizon is `hz`: windows from here, or single ticks up to a near
+// probe deadline.  On a single-GPU pool p->rc holds the counts when `can_long`.
+static int quiet_decision(gsim_pool* p, uint32_t hz, bool can_long) {
+  const GsGlobals& g = p->g;
+  const uint32_t depth = g.ring_mask + 1u;
   p->sched_counts[3]++;
   if (hz >= p->now + g.P / 2u + 1u) {
     p->quiet = true;
@@ -1968,6 +1983,8 @@ static int advance_ticks(gsim_pool* p, uint32_t chunk, bool use_graph) {
   const GsXbar* xb = p->sharded ? &p->xb : nullptr;
   uint32_t left = chunk;
   const bool can_window = windows_possible(p);
+  // sharded pools and pools without graphs look for quietness from the host, between chunks (try_quiet)
+  const bool stretch = can_window && !p->sharded && use_graph;
   while (left) {
     if (can_window && p->quiet) {
       uint32_t done = 0;
@@ -1996,6 +2013,35 @@ static int advance_ticks(gsim_pool* p, uint32_t chunk, bool use_graph) {
         p->healthy = false;
         p->pristine = false;
         p->retry_at = p->now + 1u;
+      }
+      continue;
+    }
+    if (stretch) {
+      // Single ticks up to the first quiet tick, found by the device (run_tick_stretch): one submission and
+      // one readback for the whole busy stretch, with the quiet probe behind it when it stopped quiet.
+      // A host write at tick T counts like mail at T; after a near probe deadline nobody looks before retry_at.
+      const uint32_t depth = p->g.ring_mask + 1u;
+      uint32_t floor = p->dirty_tick + 1u;
+      if (p->retry_at > floor + depth) floor = p->retry_at - depth;
+      const bool can_long = probes_always_answered(p);
+      counts_invalidate(p);
+      if (!upload_globals(p)) return GSIM_ERR_CUDA;
+      GsStretch s;
+      double tms = 0;
+      if (!be->run_tick_stretch(p->d, p->g_dev, p->g, p->now, left, floor, can_long, &tms, &s)) return GSIM_ERR_CUDA;
+      p->last_active = s.last_active;
+      p->last_ms += tms;
+      p->last_launches += s.launches;
+      p->sched_counts[5] += (uint64_t)(tms * 1e6);
+      p->sched_counts[2] += s.ran;
+      p->now += s.ran;
+      p->node_ticks += (uint64_t)s.ran * p->g.n;
+      left -= s.ran;
+      if (s.quiet) {
+        if (can_long) p->rc = s.counts;
+        p->counts_stale = !can_long;
+        int rc = quiet_decision(p, s.horizon, can_long);
+        if (rc) return rc;
       }
       continue;
     }

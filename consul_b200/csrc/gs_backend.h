@@ -24,6 +24,16 @@ struct GsRecount {
                               // still lists as alive or suspect: the targets an unanswered probe can hit
 };
 
+// What GsBackend::run_tick_stretch did: read back in one piece.
+struct GsStretch {
+  uint32_t ran;          // ticks run
+  uint32_t launches;     // tick launches, including those that found the stretch over and ran nothing
+  uint32_t last_active;  // GS_Q_LAST_ACTIVE at the end
+  uint32_t quiet;        // 1: stopped at a quiet tick, and the two fields below are set
+  uint32_t horizon;      // quiet_probe's horizon at t0 + ran
+  GsRecount counts;      // ... and its counts (when asked for)
+};
+
 // ---- device write batches -------------------------------------------------------------------
 // The host side of an operation (a new member, a join, a retired rumor) is a few dozen small writes,
 // several of them read-modify-writes of a word the host does not keep.  They are queued as an ordered
@@ -136,6 +146,31 @@ class GsBackend {
                               uint32_t* last_active) {
     return run_ticks(d, g_dev, g, t0, nticks, use_graph, kernel_ms, launches, xbar) &&
            d2h(last_active, d.qstate[g.rank] + GS_Q_LAST_ACTIVE, 4);
+  }
+  // Single ticks until the pool is quiet (DESIGN.md §4.2), single-GPU pools: tick t0 + k runs unless
+  // t0 + k >= t0 + nticks or t0 + k >= max(GS_Q_LAST_ACTIVE, floor) + depth (depth = g.ring_mask + 1: every
+  // arrival slot has been scanned empty once since the last mail).  When it stopped at such a quiet tick,
+  // out->horizon and (counts) out->counts are quiet_probe's at that tick.  The CUDA backend decides on the
+  // device and waits once; by default it is run_ticks_read one tick at a time, then quiet_probe.
+  virtual bool run_tick_stretch(const GsDev& d, const GsGlobals* g_dev, const GsGlobals& g, uint32_t t0,
+                                uint32_t nticks, uint32_t floor, bool counts, double* kernel_ms, GsStretch* out) {
+    const uint32_t depth = g.ring_mask + 1u;
+    *out = GsStretch();
+    if (!d2h(&out->last_active, d.qstate[0] + GS_Q_LAST_ACTIVE, 4)) return false;
+    for (;;) {
+      const uint32_t la = out->last_active > floor ? out->last_active : floor;
+      if (t0 + out->ran >= la + depth) {
+        out->quiet = 1u;
+        break;
+      }
+      if (out->ran == nticks) break;
+      uint64_t nl = 0;
+      if (!run_ticks_read(d, g_dev, g, t0 + out->ran, 1u, true, kernel_ms, &nl, nullptr, &out->last_active))
+        return false;
+      out->ran++;
+      out->launches++;
+    }
+    return !out->quiet || quiet_probe(d, g_dev, g, t0 + out->ran, &out->horizon, counts ? &out->counts : nullptr);
   }
   // Quiet windows (DESIGN.md §4.2): advance up to `nticks` ticks starting at t0 as a chain of launches
   // of <= ProbeInterval ticks each, on a pool whose mailboxes are known to be empty.  The chain stops at

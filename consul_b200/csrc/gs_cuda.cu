@@ -6,6 +6,7 @@
 //                       (SURVEY §7 K1+K2 fused: emit and apply are separated by the
 //                       double-buffered mailbox instead of a grid barrier)
 //   gs_advance_kernel   bumps the device tick counter at the end of a CUDA-graph chunk
+//   gs_stretch_*        drive a tick stretch: single ticks until the pool is quiet, decided on the device
 //   gs_init_kernel, gs_crash_kernel, gs_recount_kernel, gs_hash_kernel   control plane
 //
 // Launch shape of the tick: a persistent grid (SMs x resident CTAs) of 256-thread CTAs; every warp
@@ -27,6 +28,9 @@
 #define GS_BLOCK 256
 #define GS_GRAPH_TICKS 64
 #define GS_WIN_GRAPH 8   // quiet windows per CUDA graph
+#ifndef GS_STRETCH_TICKS
+#define GS_STRETCH_TICKS 16  // tick launches per pass of a tick stretch's loop (at most this many - 1 run nothing)
+#endif
 
 namespace {
 
@@ -182,6 +186,18 @@ __device__ __noinline__ void gs_row_step_call(const GsDev* dp, const GsGlobals* 
   gs_row_step_body<false>(*dp, *gp, i, t, t % gp->GI, inb, sink);
 }
 
+// Tick stretches (run_tick_stretch): the control block on the device, in the backend's scratch.
+struct GsStretchCtl {
+  GsStretch out;               // read back at the end
+  uint32_t violation;          // GS_Q_VIOLATION at the end (read back with `out`)
+  uint32_t end, floor, depth;  // ticks before `end` run until the first tick >= max(LAST_ACTIVE, floor) + depth
+};
+// the tick at which the stretch stops, given GS_Q_LAST_ACTIVE
+__device__ __forceinline__ uint32_t gs_stretch_stop(const GsStretchCtl& c, uint32_t last_active) {
+  const uint32_t quiet_at = (last_active > c.floor ? last_active : c.floor) + c.depth;
+  return quiet_at < c.end ? quiet_at : c.end;
+}
+
 // Persistent, warp-centric tick.  Every warp owns a CONTIGUOUS chunk of tiles (128 members
 // each); because ticker phases are dealt round-robin over tiles, every chunk holds the same
 // number of probing tiles (+-1) at every tick, so the static split is balanced.
@@ -196,7 +212,8 @@ __device__ __noinline__ void gs_row_step_call(const GsDev* dp, const GsGlobals* 
 // Whatever the fast path declines goes to the generic gs_row_step.
 template <bool COORDS>
 __global__ void __launch_bounds__(GS_BLOCK, GS_MIN_BLOCKS)
-    gs_tick_kernel(const __grid_constant__ GsDev d, const GsGlobals* __restrict__ gp, uint32_t k_off) {
+    gs_tick_kernel(const __grid_constant__ GsDev d, const GsGlobals* __restrict__ gp, uint32_t k_off,
+                   const GsStretchCtl* __restrict__ stretch) {
   __shared__ uint32_t s_stat[GS_NSTAT * 32];  // [counter][lane]
   __shared__ uint32_t s_heard[32 * 32];       // [broadcast slot][lane]
   __shared__ __align__(128) uint32_t s_inb[GS_WARPS][GS_ROUND][GS_TILE];  // a warp's round of mailbox words ...
@@ -221,6 +238,13 @@ __global__ void __launch_bounds__(GS_BLOCK, GS_MIN_BLOCKS)
   // this line touches no global memory.
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   asm volatile("griddepcontrol.wait;" ::: "memory");
+  // Inside a tick stretch (single-GPU pools) a launch whose tick is past the stretch's end or at its first
+  // quiet tick runs nothing: it neither scans nor publishes.  Every thread of every CTA decides the same
+  // without a barrier, although CTAs of this tick may raise GS_Q_LAST_ACTIVE while others still read it:
+  // the word only grows, and a tick that stops publishes nothing, so the only raised value a thread can
+  // read comes from a CTA of this tick that runs, and a higher LAST_ACTIVE only makes "run" more certain.
+  if (stretch != nullptr && *d.tick_base + k_off >= gs_stretch_stop(*stretch, __ldcg(d.qstate[0] + GS_Q_LAST_ACTIVE)))
+    return;
   __syncthreads();
   const GsGlobals& g = *gp;
   const uint32_t t = *d.tick_base + k_off;
@@ -858,14 +882,17 @@ __global__ void __launch_bounds__(GS_BLOCK, PRISTINE ? GS_WIN_BLOCKS_CLOSED : GS
 // Horizon of the pool as it stands (run before the first window after single ticks): the minimum,
 // over running members with a probe in flight, of the tick at which it can end in an accusation.
 __global__ void __launch_bounds__(GS_BLOCK)
-    gs_quiet_scan_kernel(GsDev d, const GsGlobals* __restrict__ gp, uint32_t now, uint32_t first, uint32_t count) {
+    gs_quiet_scan_kernel(GsDev d, const GsGlobals* __restrict__ gp, uint32_t now, const uint32_t* now_at, uint32_t first,
+                         uint32_t count) {
   __shared__ uint32_t s_min;
   if (threadIdx.x == 0u) s_min = GS_NEVER;
   __syncthreads();
   const GsGlobals& g = *gp;
+  if (now_at != nullptr) now = *now_at;  // (inside a graph: the device clock)
   uint32_t h = GS_NEVER;
   for (uint32_t x = blockIdx.x * GS_BLOCK + threadIdx.x; x < count; x += gridDim.x * GS_BLOCK) {
     const uint32_t i = first + x;
+    if (i >= g.n) break;
     if (gs_key_truth(d.key[now & 1u][i]) != GS_TRUTH_UP) continue;
     const uint32_t stage = gs_meta_stage(d.meta[i]);
     if (stage == GS_STAGE_IDLE) continue;
@@ -888,6 +915,39 @@ __global__ void gs_window_advance_kernel(uint32_t* tick_base, const uint32_t* qs
 __global__ void gs_advance_kernel(uint32_t* tick_base, uint32_t k, uint32_t* done_ctr) {
   *tick_base += k;
   if (done_ctr) *done_ctr = 0u;
+}
+
+// A tick stretch (CudaBackend::run_tick_stretch): begin, the end of each pass of its loop, and its end.
+__global__ void gs_stretch_begin_kernel(GsStretchCtl* c, uint32_t end, uint32_t floor, uint32_t depth) {
+  c->out = GsStretch();
+  c->violation = 0u;
+  c->end = end;
+  c->floor = floor;
+  c->depth = depth;
+}
+// After a pass of `k` tick launches: the device clock moves on by the ticks that ran (the launches of the
+// pass apply the same rule: every tick before the stop ran, none after it), and the loop ends at the stop.
+__global__ void gs_stretch_pass_kernel(uint32_t* tick_base, const uint32_t* qs, GsStretchCtl* c, uint32_t k,
+                                       cudaGraphConditionalHandle loop) {
+  const uint32_t t = *tick_base, la = qs[GS_Q_LAST_ACTIVE];
+  const uint32_t stop = gs_stretch_stop(*c, la);
+  const uint32_t ran = stop <= t ? 0u : stop - t < k ? stop - t : k;
+  *tick_base = t + ran;
+  c->out.ran += ran;
+  c->out.launches += k;
+  if (t + ran >= stop || qs[GS_Q_VIOLATION] != 0u) {
+    c->out.last_active = la;
+    c->out.quiet = t + ran >= (la > c->floor ? la : c->floor) + c->depth ? 1u : 0u;
+    c->violation = qs[GS_Q_VIOLATION];
+    cudaGraphSetConditional(loop, 0u);
+  }
+}
+// Stopped at a quiet tick: the quiet probe runs (horizon reset here, then scan and counts).
+__global__ void gs_stretch_end_kernel(const GsStretchCtl* c, uint32_t* qs, cudaGraphConditionalHandle probe) {
+  if (c->out.quiet && !c->violation) {
+    qs[GS_Q_HORIZON] = GS_NEVER;
+    cudaGraphSetConditional(probe, 1u);
+  }
 }
 
 // Cross-GPU barrier (sharded pools).  One warp: lane r publishes this rank's new epoch into
@@ -959,12 +1019,14 @@ __global__ void __launch_bounds__(GS_BLOCK)
 }
 
 __global__ void __launch_bounds__(GS_BLOCK)
-    gs_recount_kernel(GsDev d, const GsGlobals* __restrict__ gp, uint32_t now, uint32_t first, uint32_t count, GsRecount* out) {
+    gs_recount_kernel(GsDev d, const GsGlobals* __restrict__ gp, uint32_t now, const uint32_t* now_at, uint32_t first,
+                      uint32_t count, GsRecount* out) {
   __shared__ GsRecount s;
   uint32_t* sw = reinterpret_cast<uint32_t*>(&s);
   for (uint32_t x = threadIdx.x; x < sizeof(GsRecount) / 4; x += GS_BLOCK) sw[x] = 0u;
   __syncthreads();
   const GsGlobals& g = *gp;
+  if (now_at != nullptr) now = *now_at;  // (inside a graph: the device clock)
   const uint32_t x = blockIdx.x * GS_BLOCK + threadIdx.x, i = first + x;
   if (x < count && i < g.n) {
     uint32_t k = d.key[now & 1u][i];
@@ -1017,7 +1079,8 @@ __global__ void __launch_bounds__(GS_BLOCK)
 // Tick launches use programmatic stream serialization (PDL) so consecutive ticks overlap
 // launch latency and prologue with the previous tick's tail.
 static cudaError_t gs_launch_tick(uint32_t blocks, cudaStream_t stream, const GsDev& d,
-                                  const GsGlobals* g_dev, uint32_t k, bool pdl) {
+                                  const GsGlobals* g_dev, uint32_t k, bool pdl,
+                                  const GsStretchCtl* stretch = nullptr) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(blocks);
   cfg.blockDim = dim3(GS_BLOCK);
@@ -1028,8 +1091,8 @@ static cudaError_t gs_launch_tick(uint32_t blocks, cudaStream_t stream, const Gs
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = pdl ? 1 : 0;
-  return d.coord ? cudaLaunchKernelEx(&cfg, gs_tick_kernel<true>, d, g_dev, k)
-                 : cudaLaunchKernelEx(&cfg, gs_tick_kernel<false>, d, g_dev, k);
+  return d.coord ? cudaLaunchKernelEx(&cfg, gs_tick_kernel<true>, d, g_dev, k, stretch)
+                 : cudaLaunchKernelEx(&cfg, gs_tick_kernel<false>, d, g_dev, k, stretch);
 }
 
 static cudaError_t gs_launch_window(uint32_t blocks, cudaStream_t stream, const GsDev& d, const GsGlobals* g_dev,
@@ -1115,6 +1178,7 @@ class CudaBackend : public GsBackend {
     cudaSetDevice(dev_);
     for (auto& kv : graphs_) cudaGraphExecDestroy(kv.second);
     for (auto& kv : wgraphs_) cudaGraphExecDestroy(kv.second);
+    for (auto& kv : sgraphs_) cudaGraphExecDestroy(kv.second);
     if (sharded_) vmm_.destroy();
     if (scratch_) cudaFree(scratch_);
     cudaEventDestroy(ev0_);
@@ -1216,34 +1280,8 @@ class CudaBackend : public GsBackend {
       return d2h(last_active, d.qstate[g.rank] + GS_Q_LAST_ACTIVE, 4);
     }
     cudaSetDevice(dev_);
-    // performance variant: keep the status replica (1 byte per member, gathered at random by every
-    // prober) resident in L2 — persisting hits for the window, streaming for everything else.
-    // Set on the stream before any capture, so graph kernel nodes inherit it.
-    if (d.kst != nullptr && !l2_window_set_ && getenv("GSIM_NO_L2_WINDOW") == nullptr) {
-      l2_window_set_ = true;
-      cudaDeviceProp prop;
-      if (cudaGetDeviceProperties(&prop, dev_) == cudaSuccess && prop.persistingL2CacheMaxSize > 0) {
-        size_t bytes = g.cap;
-        if (bytes > (size_t)prop.accessPolicyMaxWindowSize) bytes = (size_t)prop.accessPolicyMaxWindowSize;
-        size_t carve = bytes < (size_t)prop.persistingL2CacheMaxSize ? bytes : (size_t)prop.persistingL2CacheMaxSize;
-        cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, carve);
-        cudaStreamAttrValue v;
-        memset(&v, 0, sizeof(v));
-        v.accessPolicyWindow.base_ptr = d.kst;
-        v.accessPolicyWindow.num_bytes = bytes;
-        v.accessPolicyWindow.hitRatio = bytes <= carve ? 1.0f : (float)carve / (float)bytes;
-        v.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
-        v.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
-        cudaStreamSetAttribute(stream_, cudaStreamAttributeAccessPolicyWindow, &v);
-        cudaGetLastError();  // best effort: an unsupported attribute must not fail the step
-      }
-    }
-    // persistent launch: one warp per 128-member tile up to a full machine (SMs x resident CTAs)
-    uint32_t tiles = (g.n + GS_TILE - 1) / GS_TILE;
-    if (g.world > 1 && tiles > g.rows_per_rank / GS_TILE) tiles = g.rows_per_rank / GS_TILE;
-    const uint32_t warps_per_block = GS_BLOCK / 32;
-    uint32_t blocks = (tiles + warps_per_block - 1) / warps_per_block;
-    if (blocks > full_grid_) blocks = full_grid_;
+    l2_window(d, g);
+    const uint32_t blocks = tick_blocks(g);
     if (!ok(cudaEventRecord(ev0_, stream_), "event")) return false;
     uint32_t left = nticks;
     if (use_graph && (!xbar || !no_shard_graph_) && left >= GS_GRAPH_TICKS) {
@@ -1277,6 +1315,40 @@ class CudaBackend : public GsBackend {
     cudaEventElapsedTime(&ms, ev0_, ev1_);
     if (kernel_ms) *kernel_ms += ms;
     if (launches) *launches += nticks;
+    if (violation != 0u) {
+      snprintf(err_, sizeof(err_), "tick %u: a bulk copy of the mailbox scan did not complete (kernel invariant broken)", violation - 1u);
+      return false;
+    }
+    return true;
+  }
+  // A tick stretch is one CUDA graph: a WHILE loop whose body is GS_STRETCH_TICKS tick launches chained with
+  // PDL plus gs_stretch_pass_kernel, which moves the clock by the ticks that ran and ends the loop at the
+  // stop; then, when the stretch stopped quiet, the quiet probe (an IF node).  The control block is set by
+  // one launch in front of the graph and read back in one copy behind it.
+  bool run_tick_stretch(const GsDev& d, const GsGlobals* g_dev, const GsGlobals& g, uint32_t t0, uint32_t nticks,
+                        uint32_t floor, bool counts, double* kernel_ms, GsStretch* out) override {
+    if (!g.n) return GsBackend::run_tick_stretch(d, g_dev, g, t0, nticks, floor, counts, kernel_ms, out);
+    cudaSetDevice(dev_);
+    l2_window(d, g);
+    cudaGraphExec_t ge = stretch_graph_for(d, g_dev, g, tick_blocks(g), counts);
+    if (!ge) return false;
+    GsStretchCtl* c = stretch_ctl();
+    if (!ok(cudaEventRecord(ev0_, stream_), "event")) return false;
+    gs_stretch_begin_kernel<<<1, 1, 0, stream_>>>(c, t0 + nticks, floor, g.ring_mask + 1u);
+    if (!ok(cudaGetLastError(), "stretch begin") || !ok(cudaGraphLaunch(ge, stream_), "stretch graph launch")) return false;
+    // (the graph records ev1_ when its loop is done: the quiet probe is not tick time)
+    uint8_t back[sizeof(GsStretch) + 4];
+    if (!ok(cudaMemcpyAsync(back, c, sizeof(back), cudaMemcpyDeviceToHost, stream_), "stretch d2h") ||
+        !ok(cudaStreamSynchronize(stream_), "stretch sync"))
+      return false;
+    memcpy(out, back, sizeof(GsStretch));
+    uint32_t violation;
+    memcpy(&violation, back + sizeof(GsStretch), 4);
+    const uint32_t passes = out->launches / GS_STRETCH_TICKS;
+    launches_ += 1u + out->launches + passes + 1u + (out->quiet ? (counts ? 3u : 2u) : 0u);
+    float ms = 0.f;
+    cudaEventElapsedTime(&ms, ev0_, ev1_);
+    if (kernel_ms) *kernel_ms += ms;
     if (violation != 0u) {
       snprintf(err_, sizeof(err_), "tick %u: a bulk copy of the mailbox scan did not complete (kernel invariant broken)", violation - 1u);
       return false;
@@ -1353,7 +1425,7 @@ class CudaBackend : public GsBackend {
     if (!count) return true;
     uint32_t blocks = (count + GS_BLOCK - 1) / GS_BLOCK;
     if (blocks > sms_ * 8u) blocks = sms_ * 8u;
-    gs_quiet_scan_kernel<<<blocks, GS_BLOCK, 0, stream_>>>(d, g_dev, now, first, count);
+    gs_quiet_scan_kernel<<<blocks, GS_BLOCK, 0, stream_>>>(d, g_dev, now, nullptr, first, count);
     ++launches_;
     (void)g;
     return ok(cudaGetLastError(), "quiet scan launch") && ok(cudaStreamSynchronize(stream_), "quiet scan");
@@ -1369,7 +1441,7 @@ class CudaBackend : public GsBackend {
     if (g.n) {
       uint32_t blocks = (g.n + GS_BLOCK - 1) / GS_BLOCK;
       if (blocks > sms_ * 8u) blocks = sms_ * 8u;
-      gs_quiet_scan_kernel<<<blocks, GS_BLOCK, 0, stream_>>>(d, g_dev, now, 0u, g.n);
+      gs_quiet_scan_kernel<<<blocks, GS_BLOCK, 0, stream_>>>(d, g_dev, now, nullptr, 0u, g.n);
       ++launches_;
     }
     gs_copy_word_kernel<<<1, 1, 0, stream_>>>(dh, qh);
@@ -1377,7 +1449,7 @@ class CudaBackend : public GsBackend {
     if (counts) {
       if (!ok(cudaMemsetAsync(dr, 0, sizeof(GsRecount), stream_), "memset")) return false;
       if (g.n) {
-        gs_recount_kernel<<<(g.n + GS_BLOCK - 1) / GS_BLOCK, GS_BLOCK, 0, stream_>>>(d, g_dev, now, 0u, g.n, dr);
+        gs_recount_kernel<<<(g.n + GS_BLOCK - 1) / GS_BLOCK, GS_BLOCK, 0, stream_>>>(d, g_dev, now, nullptr, 0u, g.n, dr);
         ++launches_;
       }
     }
@@ -1434,7 +1506,7 @@ class CudaBackend : public GsBackend {
     if (!ok(cudaMemsetAsync(dr, 0, sizeof(GsRecount), stream_), "memset")) return false;
     if (first < g.n && count) {
       if (count > g.n - first) count = g.n - first;
-      gs_recount_kernel<<<(count + GS_BLOCK - 1) / GS_BLOCK, GS_BLOCK, 0, stream_>>>(d, g_dev, now, first, count, dr);
+      gs_recount_kernel<<<(count + GS_BLOCK - 1) / GS_BLOCK, GS_BLOCK, 0, stream_>>>(d, g_dev, now, nullptr, first, count, dr);
       ++launches_;
     }
     return ok(cudaGetLastError(), "recount launch") && d2h(out, dr, sizeof(GsRecount));
@@ -1502,6 +1574,37 @@ class CudaBackend : public GsBackend {
   uint64_t total_launches() const override { return launches_; }
 
  private:
+  // performance variant: keep the status replica (1 byte per member, gathered at random by every
+  // prober) resident in L2 — persisting hits for the window, streaming for everything else.
+  // Set on the stream before any capture, so graph kernel nodes inherit it.
+  void l2_window(const GsDev& d, const GsGlobals& g) {
+    if (d.kst != nullptr && !l2_window_set_ && getenv("GSIM_NO_L2_WINDOW") == nullptr) {
+      l2_window_set_ = true;
+      cudaDeviceProp prop;
+      if (cudaGetDeviceProperties(&prop, dev_) == cudaSuccess && prop.persistingL2CacheMaxSize > 0) {
+        size_t bytes = g.cap;
+        if (bytes > (size_t)prop.accessPolicyMaxWindowSize) bytes = (size_t)prop.accessPolicyMaxWindowSize;
+        size_t carve = bytes < (size_t)prop.persistingL2CacheMaxSize ? bytes : (size_t)prop.persistingL2CacheMaxSize;
+        cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, carve);
+        cudaStreamAttrValue v;
+        memset(&v, 0, sizeof(v));
+        v.accessPolicyWindow.base_ptr = d.kst;
+        v.accessPolicyWindow.num_bytes = bytes;
+        v.accessPolicyWindow.hitRatio = bytes <= carve ? 1.0f : (float)carve / (float)bytes;
+        v.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
+        v.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
+        cudaStreamSetAttribute(stream_, cudaStreamAttributeAccessPolicyWindow, &v);
+        cudaGetLastError();  // best effort: an unsupported attribute must not fail the step
+      }
+    }
+  }
+  // persistent launch of the tick: one warp per 128-member tile up to a full machine (SMs x resident CTAs)
+  uint32_t tick_blocks(const GsGlobals& g) const {
+    uint32_t tiles = (g.n + GS_TILE - 1) / GS_TILE;
+    if (g.world > 1 && tiles > g.rows_per_rank / GS_TILE) tiles = g.rows_per_rank / GS_TILE;
+    uint32_t blocks = (tiles + GS_WARPS - 1) / GS_WARPS;
+    return blocks < full_grid_ ? blocks : full_grid_;
+  }
   cudaError_t cudaMemsetD32Async_(uint32_t* dst, uint32_t value, size_t count) {
     // the runtime API has no 32-bit memset: a grid-stride fill kernel on the pool's stream
     if (!count) return cudaSuccess;
@@ -1511,17 +1614,22 @@ class CudaBackend : public GsBackend {
     ++launches_;
     return cudaGetLastError();
   }
-  cudaGraphExec_t graph_for(const GsDev& d, const GsGlobals* g_dev, uint32_t blocks, const GsXbar* xbar) {
-    // the column pointers are baked into the captured launches: if they changed (a peer graph was
-    // attached or removed), every cached graph is stale
+  // the column pointers are baked into the captured launches: if they changed (a peer graph was
+  // attached or removed), every cached graph is stale
+  void drop_stale_graphs(const GsDev& d) {
     if (have_graph_dev_ && memcmp(&graph_dev_, &d, sizeof(GsDev)) != 0) {
       for (auto& kv : graphs_) cudaGraphExecDestroy(kv.second);
       graphs_.clear();
       for (auto& kv : wgraphs_) cudaGraphExecDestroy(kv.second);
       wgraphs_.clear();
+      for (auto& kv : sgraphs_) cudaGraphExecDestroy(kv.second);
+      sgraphs_.clear();
     }
     graph_dev_ = d;
     have_graph_dev_ = true;
+  }
+  cudaGraphExec_t graph_for(const GsDev& d, const GsGlobals* g_dev, uint32_t blocks, const GsXbar* xbar) {
+    drop_stale_graphs(d);
     auto it = graphs_.find(blocks);
     if (it != graphs_.end()) return it->second;
     cudaGraph_t graph = nullptr;
@@ -1546,15 +1654,85 @@ class CudaBackend : public GsBackend {
     graphs_[blocks] = ge;
     return ge;
   }
-  cudaGraphExec_t window_graph_for(const GsDev& d, const GsGlobals* g_dev, uint32_t blocks, uint32_t K, bool pdl, uint32_t rank) {
-    if (have_graph_dev_ && memcmp(&graph_dev_, &d, sizeof(GsDev)) != 0) {
-      for (auto& kv : graphs_) cudaGraphExecDestroy(kv.second);
-      graphs_.clear();
-      for (auto& kv : wgraphs_) cudaGraphExecDestroy(kv.second);
-      wgraphs_.clear();
+  GsStretchCtl* stretch_ctl() { return reinterpret_cast<GsStretchCtl*>(reinterpret_cast<uint8_t*>(scratch_) + 3072); }
+  // The graph of run_tick_stretch for this grid, with or without the counts in its quiet probe.
+  cudaGraphExec_t stretch_graph_for(const GsDev& d, const GsGlobals* g_dev, const GsGlobals& g, uint32_t blocks, bool counts) {
+    drop_stale_graphs(d);
+    const uint64_t key = ((uint64_t)blocks << 1) | (counts ? 1u : 0u);
+    auto it = sgraphs_.find(key);
+    if (it != sgraphs_.end()) return it->second;
+    GsStretchCtl* c = stretch_ctl();
+    uint32_t* qs = d.qstate[0];
+    cudaGraph_t graph = nullptr;
+    cudaGraphExec_t ge = nullptr;
+    if (!ok(cudaGraphCreate(&graph, 0), "stretch graph")) return nullptr;
+    cudaGraphConditionalHandle loop = 0, probe = 0;
+    cudaGraphNode_t wn = nullptr, rn = nullptr, en = nullptr, pn = nullptr;
+    cudaGraphNodeParams wp = {};
+    wp.type = cudaGraphNodeTypeConditional;
+    cudaGraphNodeParams pp = wp;
+    bool good = ok(cudaGraphConditionalHandleCreate(&loop, graph, 1u, cudaGraphCondAssignDefault), "loop handle") &&
+                ok(cudaGraphConditionalHandleCreate(&probe, graph, 0u, cudaGraphCondAssignDefault), "probe handle");
+    if (good) {
+      wp.conditional.handle = loop;
+      wp.conditional.type = cudaGraphCondTypeWhile;
+      wp.conditional.size = 1;
+      good = ok(cudaGraphAddNode(&wn, graph, nullptr, 0, &wp), "while node");
     }
-    graph_dev_ = d;
-    have_graph_dev_ = true;
+    // the loop's body: the tick launches of one pass, then the pass kernel
+    if (good && ok(cudaStreamBeginCaptureToGraph(stream_, wp.conditional.phGraph_out[0], nullptr, nullptr, 0,
+                                                 cudaStreamCaptureModeThreadLocal), "capture")) {
+      for (uint32_t k = 0; k < GS_STRETCH_TICKS && good; ++k)
+        good = ok(gs_launch_tick(blocks, stream_, d, g_dev, k, pdl_, c), "tick capture");
+      if (good) {
+        gs_stretch_pass_kernel<<<1, 1, 0, stream_>>>(d.tick_base, qs, c, GS_STRETCH_TICKS, loop);
+        good = ok(cudaGetLastError(), "pass capture");
+      }
+      cudaGraph_t body = nullptr;
+      good = ok(cudaStreamEndCapture(stream_, &body), "end capture") && good;
+    } else {
+      good = false;
+    }
+    if (good) good = ok(cudaGraphAddEventRecordNode(&rn, graph, &wn, 1, ev1_), "event node");
+    if (good) {
+      void* args[] = {&c, &qs, &probe};
+      cudaKernelNodeParams kp = {};
+      kp.func = reinterpret_cast<void*>(gs_stretch_end_kernel);
+      kp.gridDim = dim3(1);
+      kp.blockDim = dim3(1);
+      kp.kernelParams = args;
+      good = ok(cudaGraphAddKernelNode(&en, graph, &rn, 1, &kp), "end node");
+    }
+    if (good) {
+      pp.conditional.handle = probe;
+      pp.conditional.type = cudaGraphCondTypeIf;
+      pp.conditional.size = 1;
+      good = ok(cudaGraphAddNode(&pn, graph, &en, 1, &pp), "if node");
+    }
+    // the quiet probe at the tick the stretch stopped at (the device clock): scan, horizon, counts
+    if (good && ok(cudaStreamBeginCaptureToGraph(stream_, pp.conditional.phGraph_out[0], nullptr, nullptr, 0,
+                                                 cudaStreamCaptureModeThreadLocal), "capture")) {
+      uint32_t sblocks = (g.cap + GS_BLOCK - 1) / GS_BLOCK;
+      if (sblocks > sms_ * 8u) sblocks = sms_ * 8u;
+      gs_quiet_scan_kernel<<<sblocks, GS_BLOCK, 0, stream_>>>(d, g_dev, 0u, d.tick_base, 0u, g.cap);
+      gs_copy_word_kernel<<<1, 1, 0, stream_>>>(&c->out.horizon, qs + GS_Q_HORIZON);
+      if (counts)
+        gs_recount_kernel<<<(g.cap + GS_BLOCK - 1) / GS_BLOCK, GS_BLOCK, 0, stream_>>>(d, g_dev, 0u, d.tick_base, 0u, g.cap,
+                                                                                      &c->out.counts);
+      good = ok(cudaGetLastError(), "probe capture");
+      cudaGraph_t body = nullptr;
+      good = ok(cudaStreamEndCapture(stream_, &body), "end capture") && good;
+    } else {
+      good = false;
+    }
+    if (good) good = ok(cudaGraphInstantiate(&ge, graph, 0), "instantiate");
+    cudaGraphDestroy(graph);
+    if (!good) return nullptr;
+    sgraphs_[key] = ge;
+    return ge;
+  }
+  cudaGraphExec_t window_graph_for(const GsDev& d, const GsGlobals* g_dev, uint32_t blocks, uint32_t K, bool pdl, uint32_t rank) {
+    drop_stale_graphs(d);
     const uint64_t key = ((uint64_t)blocks << 32) | K;
     auto it = wgraphs_.find(key);
     if (it != wgraphs_.end()) return it->second;
@@ -1599,6 +1777,7 @@ class CudaBackend : public GsBackend {
   uint32_t win_mode_ = getenv("GSIM_WIN_CYCLIC") && atoi(getenv("GSIM_WIN_CYCLIC")) ? 2u : 0u;
   std::map<uint32_t, cudaGraphExec_t> graphs_;
   std::map<uint64_t, cudaGraphExec_t> wgraphs_;
+  std::map<uint64_t, cudaGraphExec_t> sgraphs_;  // tick stretches, by grid and whether the probe counts
   GsDev graph_dev_;
   bool have_graph_dev_ = false;
   bool l2_window_set_ = false;
