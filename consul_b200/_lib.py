@@ -118,6 +118,10 @@ SIGNATURES = [
     ("gsim_impair_many", _i32, [_P, C.POINTER(_u32), _sz, _u32, _u32]),
     ("gsim_impair_fraction", _i32, [_P, _u32, _u32, _u32, _u32, C.POINTER(_u32)]),
     ("gsim_impair_get", _i32, [_P, _u32, C.POINTER(_u32), C.POINTER(_u32)]),
+    ("gsim_pause_many", _i32, [_P, C.POINTER(_u32), _sz, _u32, C.POINTER(_u32)]),
+    ("gsim_pause_fraction", _i32, [_P, _u32, _u32, _u32, C.POINTER(_u32)]),
+    ("gsim_pause_get", _i32, [_P, _u32, C.POINTER(_u32)]),
+    ("gsim_pause_stats", _i32, [_P, C.POINTER(_u64)]),
     ("gsim_graph_set", _i32, [_P, _u32, C.POINTER(_u32), C.POINTER(_u32)]),
     ("gsim_member_reconnect_timeout_set", _i32, [_P, _u32, _u64]),
     ("gsim_coordinate_get", _i32, [_P, _u32, C.POINTER(C.c_double)]),

@@ -21,6 +21,7 @@
 #include <vector>
 
 #include "../../include/gsim.h"
+#include "gs_aux.h"
 #include "gs_backend.h"
 #include "gs_wire.h"
 #include "gs_coord.h"
@@ -173,7 +174,7 @@ struct RumorHost {
   int coalesce = 0;
 };
 struct Sched {
-  uint32_t tick, id, action;  // action 1 = shut down after Leave()
+  uint32_t tick, id, action;  // action 1 = shut down member `id` after Leave(); 2 = resume the members paused until `tick`
 };
 
 // A few host threads that stay around between calls (Members() of a large pool splits the id range over
@@ -295,6 +296,12 @@ struct gsim_pool {
   uint32_t* imp_loss = nullptr;
   uint8_t* imp_delay = nullptr;
   uint32_t n_impaired = 0;
+  // paused members (gsim_pause_*): the resume-tick column (0 = not paused) and {paused now, resumed Alive,
+  // Suspect, Dead}; the first pause allocates the column and pause_cnt_dev, a device copy of the counts that
+  // exists only so that snapshots carry them
+  uint32_t* pause_until = nullptr;
+  uint64_t* pause_cnt_dev = nullptr;
+  uint64_t pause_cnt[4] = {0, 0, 0, 0};
   // host writes to device state not yet handed to the backend (see dev()), and whether handing an
   // earlier batch over failed (reported by the API call it belonged to)
   GsWriteBatch wb = {};
@@ -1273,6 +1280,16 @@ static int set_truth(gsim_pool* p, uint32_t id, uint32_t truth) {
   return GSIM_OK;
 }
 
+// Member id is not paused any more (crashed for good, or gone): clear its resume tick.
+static bool pause_forget(gsim_pool* p, uint32_t id) {
+  if (!p->pause_cnt[0]) return true;
+  uint32_t until = 0;
+  if (!peek(p, p->pause_until, id, &until)) return false;
+  if (!until) return true;
+  p->pause_cnt[0]--;
+  return poke(p, p->pause_until, id, 0u);
+}
+
 static int refresh_after_truth_change(gsim_pool* p) {
   counts_invalidate(p);
   if (!do_recount(p)) return GSIM_ERR_CUDA;
@@ -1300,7 +1317,11 @@ extern "C" int gsim_crash_many(gsim_pool* p, const uint32_t* ids, size_t n) {
     if (ids[x] >= p->g.n) return fail(p, GSIM_ERR_NOT_FOUND, "unknown member");
     uint32_t k;
     if (!peek(p, p->d.key[p->now & 1u], ids[x], &k)) return fail(p, GSIM_ERR_CUDA, "peek");
-    if (gs_key_truth(k) != GS_TRUTH_UP) continue;
+    if (gs_key_truth(k) != GS_TRUTH_UP) {
+      // a paused member crashes for good: its resume is cancelled
+      if (gs_key_truth(k) == GS_TRUTH_CRASHED && !pause_forget(p, ids[x])) return fail(p, GSIM_ERR_CUDA, "peek");
+      continue;
+    }
     int rc = set_truth(p, ids[x], GS_TRUTH_CRASHED);
     if (rc) return fail(p, rc, "set_truth");
   }
@@ -1428,6 +1449,8 @@ extern "C" int gsim_force_leave(gsim_pool* p, uint32_t via, uint32_t target, int
   if (k != k_before) {
     if (!poke_key(p, 0, target, k) || !poke_key(p, 1, target, k)) return fail(p, GSIM_ERR_CUDA, "poke");
     if ((m & GS_META_DIRTY) && !poke(p, p->d.meta, target, m & ~GS_META_DIRTY)) return fail(p, GSIM_ERR_CUDA, "poke");
+    // a paused member that is pruned or listed Left stays gone: it will not resume
+    if (gs_key_truth(k_before) == GS_TRUTH_CRASHED && !pause_forget(p, target)) return fail(p, GSIM_ERR_CUDA, "peek");
   }
   int rc = refresh_after_truth_change(p);
   return rc ? fail(p, rc, "recount") : GSIM_OK;
@@ -1758,6 +1781,195 @@ extern "C" int gsim_impair_get(gsim_pool* p, uint32_t id, uint32_t* loss_ppm, ui
   return GSIM_OK;
 }
 
+// ---- paused members (DESIGN.md §3.6) ---------------------------------------------------------
+// The backend defaults (gs_backend.h): the columns gs_pause_row and gs_resume_row touch, copied to the host
+// behind a GsDev of host pointers, stepped there and copied back.
+namespace {
+struct HostRows {
+  std::vector<uint32_t> key0, key1, meta, due, inbox, pause;
+  std::vector<uint8_t> kst;
+  GsDev d;
+  uint32_t slot = 0;
+  bool load(GsBackend* be, const GsDev& dd, const GsGlobals& g, const uint32_t* pause_until, uint32_t t) {
+    const size_t n = g.n;
+    d = dd;
+    slot = t & g.ring_mask;
+    key0.resize(n), key1.resize(n), meta.resize(n), due.resize(n), inbox.resize(n), pause.resize(n);
+    if (!be->d2h(key0.data(), dd.key[0], n * 4) || !be->d2h(key1.data(), dd.key[1], n * 4) ||
+        !be->d2h(meta.data(), dd.meta, n * 4) || !be->d2h(due.data(), dd.due, n * 4) ||
+        !be->d2h(inbox.data(), dd.inbox[slot], n * 4) || !be->d2h(pause.data(), pause_until, n * 4))
+      return false;
+    if (dd.kst) {
+      kst.resize(n);
+      if (!be->d2h(kst.data(), dd.kst, n)) return false;
+      d.kst = kst.data();
+    }
+    d.key[0] = d.key_rep[0] = key0.data();
+    d.key[1] = d.key_rep[1] = key1.data();
+    d.meta = meta.data();
+    d.due = due.data();
+    d.inbox[slot] = inbox.data();
+    return true;
+  }
+  bool store(GsBackend* be, const GsDev& dd, const GsGlobals& g, uint32_t* pause_until) {
+    const size_t n = g.n;
+    return be->h2d(dd.key[0], key0.data(), n * 4) && be->h2d(dd.key[1], key1.data(), n * 4) &&
+           be->h2d(dd.meta, meta.data(), n * 4) && be->h2d(dd.due, due.data(), n * 4) &&
+           be->h2d(dd.inbox[slot], inbox.data(), n * 4) && be->h2d(pause_until, pause.data(), n * 4) &&
+           (!dd.kst || be->h2d(dd.kst, kst.data(), n));
+  }
+};
+}  // namespace
+
+bool GsBackend::pause_rows(const GsDev& d, const GsGlobals*, const GsGlobals& g, uint32_t* pause_until,
+                           const uint32_t* ids, uint32_t n, uint32_t thr, uint32_t salt, uint32_t until,
+                           uint32_t* n_paused) {
+  *n_paused = 0;
+  if (!g.n) return true;
+  HostRows h;
+  if (!h.load(this, d, g, pause_until, 0u)) return false;
+  if (ids) {
+    for (uint32_t x = 0; x < n; ++x) *n_paused += gs_pause_row(h.d, g, h.pause.data(), ids[x], until) ? 1u : 0u;
+  } else {
+    for (uint32_t i = 0; i < g.n; ++i)
+      if (gs_pause_pick(g, i, thr, salt)) *n_paused += gs_pause_row(h.d, g, h.pause.data(), i, until) ? 1u : 0u;
+  }
+  return h.store(this, d, g, pause_until);
+}
+
+bool GsBackend::resume_rows(const GsDev& d, const GsGlobals*, const GsGlobals& g, uint32_t* pause_until, uint32_t t,
+                            bool resume, bool log_events, uint32_t counts[4]) {
+  counts[0] = counts[1] = counts[2] = counts[3] = 0u;
+  if (!g.n) return true;
+  HostRows h;
+  if (!h.load(this, d, g, pause_until, t)) return false;
+  std::vector<uint32_t> back_from_dead;
+  for (uint32_t i = 0; i < g.n; ++i) {
+    const uint32_t r = gs_resume_row(h.d, g, h.pause.data(), i, t, resume);
+    if (r) counts[r - 1u]++;
+    if (r == GS_RESUMED_DEAD && log_events) back_from_dead.push_back(i);
+  }
+  if (!h.store(this, d, g, pause_until)) return false;
+  if (back_from_dead.empty()) return true;
+  uint32_t cur[2];
+  if (!d2h(cur, d.evlog_cursor, 8)) return false;
+  for (uint32_t i : back_from_dead) {
+    if (cur[0] < g.evlog_cap) {
+      const GsEventRec e = {t, GS_EV_MEMBER_JOIN, i, GS_EMPTY32, 0u, 0u};
+      if (!h2d(d.evlog + cur[0], &e, sizeof(e))) return false;
+      cur[0]++;
+    } else {
+      cur[1]++;
+    }
+  }
+  return h2d(d.evlog_cursor, cur, 8);
+}
+
+static bool pause_alloc(gsim_pool* p) {
+  if (p->pause_until) return true;
+  uint32_t* col = nullptr;
+  uint64_t* cnt = nullptr;
+  if (!alloc_col(p, &col, p->g.cap) || !alloc_col(p, &cnt, 4)) return false;
+  if (!dev(p)->fill32(col, 0u, p->g.cap) || !dev(p)->fill32(reinterpret_cast<uint32_t*>(cnt), 0u, 8)) return false;
+  p->pause_until = col;
+  p->pause_cnt_dev = cnt;
+  return true;
+}
+
+static int pause_check(gsim_pool* p, uint32_t ticks) {
+  if (p->sharded) return fail(p, GSIM_ERR_STATE, "pausing members is not supported on sharded pools");
+  if (ticks == 0u) return fail(p, GSIM_ERR_INVALID, "ticks must be >= 1");
+  if (ticks >= GS_NEVER - p->now) return fail(p, GSIM_ERR_INVALID, "the resume tick must fit in 32 bits");
+  return GSIM_OK;
+}
+
+// The selected members (ids[0..n), or the draw below thr) stop now and resume at now + ticks: one resume
+// entry in the schedule per distinct tick, which also makes gsim_step end its chunks (windows, tick
+// stretches) there.
+static int pause_run(gsim_pool* p, const uint32_t* ids, uint32_t n, uint32_t thr, uint32_t salt, uint32_t ticks,
+                     uint32_t* n_paused) {
+  if (!pause_alloc(p)) return fail(p, GSIM_ERR_NOMEM, "pause column");
+  if (!upload_globals(p)) return fail(p, GSIM_ERR_CUDA, "upload");
+  mark_dirty(p);
+  const uint32_t until = p->now + ticks;
+  uint32_t k = 0;
+  if (!dev(p)->pause_rows(p->d, p->g_dev, p->g, p->pause_until, ids, n, thr, salt, until, &k))
+    return fail(p, GSIM_ERR_CUDA, "pause_rows");
+  *n_paused = k;
+  if (!k) return GSIM_OK;
+  p->pause_cnt[0] += k;
+  bool have = false;
+  for (const Sched& s : p->sched) have = have || (s.action == 2u && s.tick == until);
+  if (!have) p->sched.push_back(Sched{until, 0u, 2u});
+  int rc = refresh_after_truth_change(p);
+  return rc ? fail(p, rc, "recount") : GSIM_OK;
+}
+
+// Tick p->now, before it runs: the members whose pause ends now resume (resume = true), and the pauses of
+// members that are gone meanwhile are forgotten.  Returns whether anybody's truth changed.
+static int pause_resume(gsim_pool* p, bool resume, bool* any) {
+  uint32_t c[4];
+  if (!upload_globals(p)) return GSIM_ERR_CUDA;
+  mark_dirty(p);
+  if (!dev(p)->resume_rows(p->d, p->g_dev, p->g, p->pause_until, p->now, resume,
+                           (p->cfg.flags & GSIM_FLAG_LOG_GLOBAL_EVENTS) != 0, c))
+    return GSIM_ERR_CUDA;
+  p->pause_cnt[0] -= (uint64_t)c[0] + c[1] + c[2] + c[3];
+  for (int x = 0; x < 3; ++x) p->pause_cnt[1 + x] += c[x];
+  *any = *any || c[0] + c[1] + c[2] != 0u;
+  return GSIM_OK;
+}
+
+extern "C" int gsim_pause_many(gsim_pool* p, const uint32_t* ids, size_t n, uint32_t ticks, uint32_t* n_paused) {
+  if (!p || (!ids && n)) return GSIM_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(p->mu);
+  uint32_t local = 0;
+  if (!n_paused) n_paused = &local;
+  *n_paused = 0;
+  return controller_call(p, n_paused, sizeof(uint32_t), [&]() -> int {
+    int rc = pause_check(p, ticks);
+    if (rc) return rc;
+    std::vector<uint32_t> v(ids, ids + n);
+    for (uint32_t id : v)
+      if (id >= p->g.n) return fail(p, GSIM_ERR_NOT_FOUND, "unknown member");
+    std::sort(v.begin(), v.end());  // (the CUDA kernel takes one row per thread: no id twice)
+    v.erase(std::unique(v.begin(), v.end()), v.end());
+    if (v.empty()) return GSIM_OK;
+    return pause_run(p, v.data(), (uint32_t)v.size(), 0u, 0u, ticks, n_paused);
+  });
+}
+
+extern "C" int gsim_pause_fraction(gsim_pool* p, uint32_t member_ppm, uint32_t salt, uint32_t ticks,
+                                   uint32_t* n_paused) {
+  if (!p || member_ppm > 1000000u) return GSIM_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(p->mu);
+  uint32_t local = 0;
+  if (!n_paused) n_paused = &local;
+  *n_paused = 0;
+  return controller_call(p, n_paused, sizeof(uint32_t), [&]() -> int {
+    int rc = pause_check(p, ticks);
+    if (rc) return rc;
+    return pause_run(p, nullptr, 0u, ppm_to_thr(member_ppm), salt, ticks, n_paused);
+  });
+}
+
+extern "C" int gsim_pause_get(gsim_pool* p, uint32_t id, uint32_t* resume_tick) {
+  if (!p) return GSIM_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(p->mu);
+  if (id >= p->g.n) return fail(p, GSIM_ERR_NOT_FOUND, "unknown member");
+  uint32_t until = 0;
+  if (p->pause_until && !peek(p, p->pause_until, id, &until)) return fail(p, GSIM_ERR_CUDA, "peek");
+  if (resume_tick) *resume_tick = until ? until : 0xFFFFFFFFu;
+  return GSIM_OK;
+}
+
+extern "C" int gsim_pause_stats(gsim_pool* p, uint64_t out[4]) {
+  if (!p || !out) return GSIM_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(p->mu);
+  memcpy(out, p->pause_cnt, sizeof(p->pause_cnt));
+  return GSIM_OK;
+}
+
 // WAN latency pools (BASELINE config 5, SURVEY 8d C5): n_dcs synthetic datacenters, member i
 // lives in datacenter (i / 128) % n_dcs; a packet from datacenter a to b takes lat[a*n_dcs+b]
 // ticks (>= 1; 1 is the latency every packet has on a pool without a matrix).
@@ -1785,9 +1997,10 @@ extern "C" int gsim_latency_set(gsim_pool* p, uint32_t n_dcs, const uint8_t* lat
 
 // ---- time -----------------------------------------------------------------------
 static int apply_sched(gsim_pool* p) {
-  bool any = false;
+  bool any = false, resume = false;
   for (size_t x = 0; x < p->sched.size();) {
     if (p->sched[x].tick <= p->now) {
+      resume = resume || p->sched[x].action == 2u;
       if (p->sched[x].action == 1u) {
         uint32_t k;
         if (!peek(p, p->d.key[p->now & 1u], p->sched[x].id, &k)) return GSIM_ERR_CUDA;
@@ -1801,6 +2014,10 @@ static int apply_sched(gsim_pool* p) {
     } else {
       ++x;
     }
+  }
+  if (resume && p->pause_until) {
+    int rc = pause_resume(p, true, &any);
+    if (rc) return rc;
   }
   if (any) return refresh_after_truth_change(p);
   return GSIM_OK;
@@ -1852,6 +2069,11 @@ static int reap_pass(gsim_pool* p) {
     return GSIM_ERR_CUDA;
   if (!counts[0]) return GSIM_OK;
   p->n_established -= counts[1];
+  if (p->pause_cnt[0]) {  // a reaped member that was paused stays gone
+    bool any = false;
+    int rc = pause_resume(p, false, &any);
+    if (rc) return rc;
+  }
   return refresh_after_truth_change(p);
 }
 
@@ -2524,7 +2746,7 @@ struct SnapCol {
   uint32_t planes;   // equally sized, each a multiple of 4 bytes
   bool may_fill;     // planes may be stored as a repeated word
 };
-static std::vector<SnapCol> snap_cols(gsim_pool* p, bool with_impairment) {
+static std::vector<SnapCol> snap_cols(gsim_pool* p, bool with_impairment, bool with_pause) {
   const GsDev& d = p->d;
   const size_t cap = p->g.cap;
   std::vector<SnapCol> v;
@@ -2552,6 +2774,10 @@ static std::vector<SnapCol> snap_cols(gsim_pool* p, bool with_impairment) {
     add(p->imp_loss, cap * 4);
     add(p->imp_delay, cap);
   }
+  if (with_pause) {
+    add(p->pause_until, cap * 4);
+    add(p->pause_cnt_dev, 4 * 8, 1, false);
+  }
   add(d.stats, GSIM_STAT_COUNT * 8, 1, false); add(d.heard_cnt, 32 * 4, 1, false); add(d.conv_tick, 32 * 4, 1, false);
   add(d.crashed_alive, 4, 1, false); add(d.crashed_dead_tick, 4, 1, false);
   return v;
@@ -2578,6 +2804,7 @@ static uint32_t snap_layout(const gsim_pool* p) {
   if (p->d.kst) m |= 4u;
   if (p->imp_loss) m |= 8u;  // impairment columns (restore allocates them when the pool has none)
   if (p->sharded) m |= 16u;
+  if (p->pause_until) m |= 32u;  // the pause column and statistics (restore allocates them when the pool has none)
   return m;
 }
 static uint64_t snap_graph_hash(const gsim_pool* p) {
@@ -2597,7 +2824,7 @@ static uint64_t snap_graph_hash(const gsim_pool* p) {
 static size_t snap_size(gsim_pool* p) {
   size_t s = sizeof(SnapHeader) + p->sched.size() * sizeof(Sched);
   for (uint32_t r = 0; r < GS_MAX_RUMORS; ++r) s += 12 + p->rh[r].name.size() + p->rh[r].payload.size();
-  for (const SnapCol& c : snap_cols(p, p->imp_loss != nullptr)) s += c.bytes + 4u * c.planes;  // upper bound: every plane raw
+  for (const SnapCol& c : snap_cols(p, p->imp_loss != nullptr, p->pause_until != nullptr)) s += c.bytes + 4u * c.planes;  // upper bound: every plane raw
   return s;
 }
 
@@ -2644,7 +2871,9 @@ extern "C" int gsim_snapshot(gsim_pool* p, void* out, size_t cap_bytes, size_t* 
     memcpy(w, p->rh[r].payload.data(), hdr[1]);
     w += hdr[1];
   }
-  for (const SnapCol& c : snap_cols(p, p->imp_loss != nullptr)) {
+  if (p->pause_cnt_dev && !dev(p)->h2d(p->pause_cnt_dev, p->pause_cnt, sizeof(p->pause_cnt)))
+    return fail(p, GSIM_ERR_CUDA, "h2d");
+  for (const SnapCol& c : snap_cols(p, p->imp_loss != nullptr, p->pause_until != nullptr)) {
     const size_t pb = c.bytes / c.planes;
     for (uint32_t q = 0; q < c.planes; ++q) {
       uint8_t* raw = w + 4;
@@ -2674,7 +2903,7 @@ extern "C" int gsim_restore(gsim_pool* p, const void* blob, size_t n_bytes) {
   // geometry and peer graph must be this pool's before a single plane is copied.
   if (h.cap != p->g.cap || h.g.cap != p->g.cap || h.g.n > p->cfg.capacity || h.g.n > p->g.cap ||
       h.g.ring_mask != p->g.ring_mask || (h.g.pp_interval != 0u) != (p->g.pp_interval != 0u) ||
-      (h.layout & ~8u) != (snap_layout(p) & ~8u) || h.g.world != p->g.world || h.g.key_stride != p->g.key_stride ||
+      (h.layout & ~40u) != (snap_layout(p) & ~40u) || h.g.world != p->g.world || h.g.key_stride != p->g.key_stride ||
       h.g.rows_per_rank != p->g.rows_per_rank || h.g.phase_group != p->g.phase_group ||
       h.g.graph_n != p->g.graph_n || h.graph_hash != snap_graph_hash(p) || h.n_established > h.g.n)
     return fail(p, GSIM_ERR_INVALID, "snapshot does not match this pool (capacity, column set, sharding or peer graph)");
@@ -2696,7 +2925,9 @@ extern "C" int gsim_restore(gsim_pool* p, const void* blob, size_t n_bytes) {
   }
   const bool blob_impaired = (h.layout & 8u) != 0u;
   if (blob_impaired && !impair_alloc(p)) return fail(p, GSIM_ERR_NOMEM, "impairment columns");
-  for (const SnapCol& c : snap_cols(p, blob_impaired)) {
+  const bool blob_paused = (h.layout & 32u) != 0u;
+  if (blob_paused && !pause_alloc(p)) return fail(p, GSIM_ERR_NOMEM, "pause column");
+  for (const SnapCol& c : snap_cols(p, blob_impaired, blob_paused)) {
     if (c.may_fill) {  // plane by plane: a device fill or a copy
       const size_t pb = c.bytes / c.planes;
       for (uint32_t q = 0; q < c.planes; ++q) {
@@ -2739,7 +2970,11 @@ extern "C" int gsim_restore(gsim_pool* p, const void* blob, size_t n_bytes) {
   if (!blob_impaired && p->imp_loss &&
       (!dev(p)->fill32(p->imp_loss, 0, p->g.cap) || !dev(p)->fill8(p->imp_delay, 0, p->g.cap)))
     return fail(p, GSIM_ERR_CUDA, "fill");
+  // ... and one without the pause column a pool nobody in it is paused
+  if (!blob_paused && p->pause_until && !dev(p)->fill32(p->pause_until, 0u, p->g.cap)) return fail(p, GSIM_ERR_CUDA, "fill");
   if (!dev(p)->sync()) return fail(p, GSIM_ERR_CUDA, "sync");  // every plane has left the caller's blob
+  memset(p->pause_cnt, 0, sizeof(p->pause_cnt));
+  if (blob_paused && !dev(p)->d2h(p->pause_cnt, p->pause_cnt_dev, sizeof(p->pause_cnt))) return fail(p, GSIM_ERR_CUDA, "d2h");
   {
     // topology fields stay the live pool's (they were checked equal above, except the rank, which is
     // this process's own on a sharded pool)

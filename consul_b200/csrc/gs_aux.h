@@ -69,6 +69,58 @@ GS_DEV bool gs_crash_row(const GsDev& d, const GsGlobals& g, uint32_t i, uint32_
   return true;
 }
 
+// ---- paused members (gsim_pause_*, DESIGN.md §3.6) ---------------------------------------------
+// pause_until[i] = the tick member i resumes at, 0 = not paused.  While paused its truth is CRASHED: every
+// kernel treats it as it treats a crashed process.
+
+// gsim_pause_fraction's draw for member i: its own purpose word, so the selection is independent of the
+// crash and impairment selections for the same salt.
+GS_DEV bool gs_pause_pick(const GsGlobals& g, uint32_t i, uint32_t thr, uint32_t salt) {
+  return gs_philox(g.seed_lo, g.seed_hi, i, salt, GS_PUR_PAUSE, 0u).x < thr;
+}
+
+// Pause member i until tick `until` if it runs and is not leaving (a leaving member's scheduled shutdown
+// only fires for a running process).  A paused member is not running, so it is never paused twice.
+GS_DEV bool gs_pause_row(const GsDev& d, const GsGlobals& g, uint32_t* pause_until, uint32_t i, uint32_t until) {
+  const uint32_t k0 = d.key[0][i];
+  if (gs_key_truth(k0) != GS_TRUTH_UP || (d.meta[i] & GS_META_LEAVING)) return false;
+  gs_key_store(d, g, 0u, i, (k0 & ~3u) | GS_TRUTH_CRASHED);
+  gs_key_store(d, g, 1u, i, (d.key[1][i] & ~3u) | GS_TRUTH_CRASHED);
+  pause_until[i] = until;
+  return true;
+}
+
+// Resume codes of gs_resume_row (0 = nothing to do).
+enum { GS_RESUMED_ALIVE = 1, GS_RESUMED_SUSPECT = 2, GS_RESUMED_DEAD = 3, GS_PAUSE_FORGOTTEN = 4 };
+
+// Tick t, before it runs (resume = true): member i resumes if its pause ends now.  The process carries on
+// with the state it had: truth goes back to UP in both key buffers and nothing else of the member's state
+// changes, except that a probe in flight is abandoned (stage IDLE, no missed nacks) and its ticker fires next
+// at the first tick >= t on its phase (a `due` off the phase would never fire, gs_tile_probe_gate).  A wake
+// in the slot tick t reads steps the row at once: section B refutes a Suspect or Dead record, and a member
+// with broadcasts queued has its wake again (the GS_WAKE_BIT invariant).  Returns the rank it comes back to.
+// A paused member that is gone (reaped, pruned, or listed Left by force_leave) never resumes: its pause is
+// forgotten (GS_PAUSE_FORGOTTEN), at its resume tick or by a sweep with resume = false.
+GS_DEV uint32_t gs_resume_row(const GsDev& d, const GsGlobals& g, uint32_t* pause_until, uint32_t i, uint32_t t,
+                              bool resume) {
+  const uint32_t until = pause_until[i];
+  if (until == 0u) return 0u;
+  const uint32_t k = d.key[t & 1u][i];
+  if (gs_key_truth(k) == GS_TRUTH_CRASHED && gs_key_rank(k) != GS_RANK_LEFT) {
+    if (!resume || until != t) return 0u;
+    gs_key_store(d, g, 0u, i, (d.key[0][i] & ~3u) | GS_TRUTH_UP);
+    gs_key_store(d, g, 1u, i, (d.key[1][i] & ~3u) | GS_TRUTH_UP);
+    d.meta[i] = gs_meta_set_nmiss(gs_meta_set_stage(d.meta[i], GS_STAGE_IDLE), 0u);
+    const uint32_t pp = gs_probe_phase(g.rot_p, i / g.phase_group, g.P);
+    d.due[i] = t + (pp + g.P - t % g.P) % g.P;
+    d.inbox[t & g.ring_mask][i] |= GS_WAKE_BIT;
+    pause_until[i] = 0u;
+    return GS_RESUMED_ALIVE + gs_key_rank(k);
+  }
+  pause_until[i] = 0u;
+  return GS_PAUSE_FORGOTTEN;
+}
+
 // [U] serf.handleReap -> reap(failedMembers, ReconnectTimeout) / reap(leftMembers, TombstoneTimeout):
 // a member that has been Failed (Left) for longer than the timeout is erased from the member
 // list (EventMemberReap).  Row a17 of SURVEY 8a; Consul shortens the timeouts in

@@ -223,6 +223,18 @@ class GsBackend {
     }
     return h2d(loss_col, lc.data(), (size_t)g.n * 4) && h2d(delay_col, dc.data(), g.n);
   }
+  // Paused members (gs_aux.h; pause_until is the caller's column).  pause_rows: gs_pause_row(until) over the
+  // `n` distinct members ids[] when ids != nullptr, otherwise over every member whose gs_pause_pick(thr, salt)
+  // draw selects it; *n_paused = members paused.  resume_rows: gs_resume_row(t, resume) over every member,
+  // logging a pool-wide EventMemberJoin at t for each member that comes back from Dead when `log_events`;
+  // counts[0..2] = resumed Alive / Suspect / Dead, counts[3] = pauses forgotten.  Both are defined in
+  // gs_api.cpp through the copy primitives every backend has, which is what the host emulation runs; the CUDA
+  // backend replaces them with one kernel each.
+  virtual bool pause_rows(const GsDev& d, const GsGlobals* g_dev, const GsGlobals& g, uint32_t* pause_until,
+                          const uint32_t* ids, uint32_t n, uint32_t thr, uint32_t salt, uint32_t until,
+                          uint32_t* n_paused);
+  virtual bool resume_rows(const GsDev& d, const GsGlobals* g_dev, const GsGlobals& g, uint32_t* pause_until,
+                           uint32_t t, bool resume, bool log_events, uint32_t counts[4]);
   // counts over members [first, first + count) (a rank of a sharded pool counts its own rows)
   virtual bool recount(const GsDev& d, const GsGlobals* g_dev, const GsGlobals& g, uint32_t now, uint32_t first,
                        uint32_t count, GsRecount* out) = 0;

@@ -63,7 +63,8 @@ enum {
   GS_PUR_CRASH = 6,
   GS_PUR_PUSHPULL = 7,
   // 8 = GS_PUR_COORD (gs_coord.h)
-  GS_PUR_IMPAIR = 9
+  GS_PUR_IMPAIR = 9,
+  GS_PUR_PAUSE = 10
 };
 // Loss "kind" (folded into the counter) — one draw per simulated UDP packet.
 enum {

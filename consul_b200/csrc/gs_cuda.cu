@@ -8,6 +8,7 @@
 //   gs_advance_kernel   bumps the device tick counter at the end of a CUDA-graph chunk
 //   gs_stretch_*        drive a tick stretch: single ticks until the pool is quiet, decided on the device
 //   gs_init_kernel, gs_crash_kernel, gs_recount_kernel, gs_hash_kernel   control plane
+//   gs_pause_kernel, gs_resume_kernel   paused members (gsim_pause_*, DESIGN.md §3.6)
 //
 // Launch shape of the tick: a persistent grid (SMs x resident CTAs) of 256-thread CTAs; every warp
 // owns a contiguous chunk of 128-member tiles, scans their 4-byte mailbox words through a
@@ -1001,6 +1002,41 @@ __global__ void __launch_bounds__(GS_BLOCK)
   }
 }
 
+// gsim_pause_many (ids != nullptr: thread x takes member ids[x], no id twice) and gsim_pause_fraction (thread i
+// takes member i): gs_pause_row, *n_paused += members paused.
+__global__ void __launch_bounds__(GS_BLOCK)
+    gs_pause_kernel(GsDev d, const GsGlobals* __restrict__ gp, uint32_t* pause_until, const uint32_t* __restrict__ ids,
+                    uint32_t n, uint32_t thr, uint32_t salt, uint32_t until, uint32_t* n_paused) {
+  const uint32_t x = blockIdx.x * GS_BLOCK + threadIdx.x;
+  const GsGlobals& g = *gp;
+  bool c = false;
+  if (ids != nullptr) {
+    if (x < n) c = gs_pause_row(d, g, pause_until, ids[x], until);
+  } else if (x < g.n && gs_pause_pick(g, x, thr, salt)) {
+    c = gs_pause_row(d, g, pause_until, x, until);
+  }
+  const unsigned b = __ballot_sync(0xFFFFFFFFu, c);
+  if ((threadIdx.x & 31u) == 0u && b) atomicAdd(n_paused, (uint32_t)__popc(b));
+}
+
+// gs_resume_row over every member at tick t; counts[c - 1] += members with resume code c.
+__global__ void __launch_bounds__(GS_BLOCK)
+    gs_resume_kernel(GsDev d, const GsGlobals* __restrict__ gp, uint32_t* pause_until, uint32_t t, uint32_t resume,
+                     uint32_t log_events, uint32_t* counts) {
+  const uint32_t i = blockIdx.x * GS_BLOCK + threadIdx.x;
+  uint32_t r = 0u;
+  if (i < gp->n) r = gs_resume_row(d, *gp, pause_until, i, t, resume != 0u);
+  if (r == GS_RESUMED_DEAD && log_events) {  // serf's handleNodeJoin of a Failed member
+    DevSink sink{nullptr, nullptr, nullptr};
+    sink.log_event(d, *gp, t, GS_EV_MEMBER_JOIN, i, GS_EMPTY32, 0u);
+  }
+  if (__ballot_sync(0xFFFFFFFFu, r != 0u) == 0u) return;
+  for (uint32_t c = 0; c < 4u; ++c) {
+    const unsigned b = __ballot_sync(0xFFFFFFFFu, r == c + 1u);
+    if ((threadIdx.x & 31u) == 0u && b) atomicAdd(&counts[c], (uint32_t)__popc(b));
+  }
+}
+
 __global__ void __launch_bounds__(GS_BLOCK)
     gs_reap_kernel(GsDev d, const GsGlobals* __restrict__ gp, uint32_t now, uint32_t reconnect_ticks,
                    uint32_t tombstone_ticks, uint32_t log_events, uint32_t* counts) {
@@ -1485,6 +1521,42 @@ class CudaBackend : public GsBackend {
       ++launches_;
     }
     return ok(cudaGetLastError(), "impair launch") && d2h(counts, cnt, 8);
+  }
+  bool pause_rows(const GsDev& d, const GsGlobals* g_dev, const GsGlobals& g, uint32_t* pause_until,
+                  const uint32_t* ids, uint32_t n, uint32_t thr, uint32_t salt, uint32_t until,
+                  uint32_t* n_paused) override {
+    cudaSetDevice(dev_);
+    uint32_t* cnt = reinterpret_cast<uint32_t*>(scratch_);
+    if (!ok(cudaMemsetAsync(cnt, 0, 4, stream_), "memset")) return false;
+    const uint32_t rows = ids ? n : g.n;
+    uint32_t* dids = nullptr;
+    if (ids && n) {  // the id list travels with the launch (pageable source: copied before the call returns)
+      if (!ok(cudaMallocAsync(reinterpret_cast<void**>(&dids), (size_t)n * 4, stream_), "malloc")) return false;
+      if (!ok(cudaMemcpyAsync(dids, ids, (size_t)n * 4, cudaMemcpyHostToDevice, stream_), "h2d")) {
+        cudaFreeAsync(dids, stream_);
+        return false;
+      }
+    }
+    if (rows) {
+      gs_pause_kernel<<<(rows + GS_BLOCK - 1) / GS_BLOCK, GS_BLOCK, 0, stream_>>>(d, g_dev, pause_until, dids, n, thr,
+                                                                                 salt, until, cnt);
+      ++launches_;
+    }
+    const bool launched = ok(cudaGetLastError(), "pause launch");
+    if (dids) cudaFreeAsync(dids, stream_);
+    return launched && d2h(n_paused, cnt, 4);
+  }
+  bool resume_rows(const GsDev& d, const GsGlobals* g_dev, const GsGlobals& g, uint32_t* pause_until, uint32_t t,
+                   bool resume, bool log_events, uint32_t counts[4]) override {
+    cudaSetDevice(dev_);
+    uint32_t* cnt = reinterpret_cast<uint32_t*>(scratch_);
+    if (!ok(cudaMemsetAsync(cnt, 0, 16, stream_), "memset")) return false;
+    if (g.n) {
+      gs_resume_kernel<<<(g.n + GS_BLOCK - 1) / GS_BLOCK, GS_BLOCK, 0, stream_>>>(
+          d, g_dev, pause_until, t, resume ? 1u : 0u, log_events ? 1u : 0u, cnt);
+      ++launches_;
+    }
+    return ok(cudaGetLastError(), "resume launch") && d2h(counts, cnt, 16);
   }
   bool reap_rows(const GsDev& d, const GsGlobals* g_dev, const GsGlobals& g, uint32_t now,
                  uint32_t reconnect_ticks, uint32_t tombstone_ticks, bool log_events,

@@ -202,6 +202,31 @@ class Pool:
         self._ck(self.lib.gsim_impair_get(self.h, member, C.byref(loss), C.byref(delay)))
         return loss.value, delay.value
 
+    def pause(self, ids, ticks: int) -> int:
+        """Stop the listed members (running, not leaving) for `ticks` ticks; returns how many were paused."""
+        arr = (C.c_uint32 * max(1, len(ids)))(*ids)
+        out = C.c_uint32()
+        self._ck(self.lib.gsim_pause_many(self.h, arr, len(ids), ticks, C.byref(out)))
+        return out.value
+
+    def pause_fraction(self, member_ppm: int, salt: int, ticks: int) -> int:
+        """Stop a seeded fraction (ppm) of the running members for `ticks` ticks; returns how many."""
+        out = C.c_uint32()
+        self._ck(self.lib.gsim_pause_fraction(self.h, member_ppm, salt, ticks, C.byref(out)))
+        return out.value
+
+    def paused_until(self, member: int) -> int:
+        """The tick the member resumes at, NEVER when it is not paused."""
+        out = C.c_uint32()
+        self._ck(self.lib.gsim_pause_get(self.h, member, C.byref(out)))
+        return out.value
+
+    def pause_stats(self):
+        """{'paused', 'resumed_alive', 'resumed_suspect', 'resumed_dead'}"""
+        out = (C.c_uint64 * 4)()
+        self._ck(self.lib.gsim_pause_stats(self.h, out))
+        return dict(zip(("paused", "resumed_alive", "resumed_suspect", "resumed_dead"), out))
+
     # -- time ---------------------------------------------------------------------
     def step(self, ticks: int = 1):
         self._ck(self.lib.gsim_step(self.h, ticks))

@@ -304,6 +304,36 @@ int gsim_impair_fraction(gsim_pool* p, uint32_t member_ppm, uint32_t salt, uint3
 /* The impairment of member `id` exactly as it was set. */
 int gsim_impair_get(gsim_pool* p, uint32_t id, uint32_t* loss_ppm, uint32_t* delay_ticks);
 
+/* Paused members (simulator-only fault injection: a GC pause, a VM steal, a SIGSTOP; DESIGN.md §3.6):
+ * a member paused at tick t0 for d ticks is a stopped process during ticks t0 .. t0+d-1 and carries on
+ * with the state it had at t0+d.
+ *  - Only members that run and are not leaving are paused; others (crashed, gone, already paused, LEAVING)
+ *    are skipped.  While paused a member's truth is GSIM_TRUTH_CRASHED, so it counts in
+ *    gsim_stats.n_crashed and in GSIM_PRED_CRASHED_ALL_DEAD, takes no probe, gossip, ack, push-pull answer
+ *    or refutation, and mail to it is lost (not held in a socket buffer).
+ *  - Resume at t0+d, before that tick runs: truth UP again, incarnation, clocks, broadcast queue and
+ *    awareness as they were; a probe in flight is abandoned (not failed) and the probe ticker fires next
+ *    at the first tick >= t0+d on its phase.  A Suspect or Dead record is refuted in tick t0+d.  One that
+ *    was Dead logs a pool-wide GSIM_EVENT_MEMBER_JOIN at t0+d when GSIM_FLAG_LOG_GLOBAL_EVENTS is set.
+ *  - gsim_crash* on a paused member cancels its resume.  A paused member that is reaped, or pruned or
+ *    listed Left by gsim_force_leave, stays gone.  gsim_leave, gsim_join, gsim_user_event and
+ *    gsim_member_update on it return GSIM_ERR_STATE like on any member that is not running.
+ *  - The resume tick column (4 bytes per member) is allocated by the first pause call; members added
+ *    later start unpaused.  Pausing is not part of gsim_state_hash (truth is); gsim_snapshot carries it
+ *    once the column exists.  Single-GPU pools only (GSIM_ERR_STATE when sharded).
+ *  - GSIM_ERR_INVALID: ticks == 0 (or a resume tick past 2^32 - 2), member_ppm > 1e6.
+ *    GSIM_ERR_NOT_FOUND: an id that was never created. */
+/* Pause the listed members for `ticks` ticks; *n_paused = how many were paused (may be NULL). */
+int gsim_pause_many(gsim_pool* p, const uint32_t* ids, size_t n, uint32_t ticks, uint32_t* n_paused);
+/* Pause every running, non-leaving member i with philox(seed; i, salt, PAUSE).x < member_ppm * 2^32 / 1e6
+ * (a selection independent of gsim_crash_fraction's and gsim_impair_fraction's for the same salt). */
+int gsim_pause_fraction(gsim_pool* p, uint32_t member_ppm, uint32_t salt, uint32_t ticks, uint32_t* n_paused);
+/* The tick member `id` resumes at, UINT32_MAX when it is not paused. */
+int gsim_pause_get(gsim_pool* p, uint32_t id, uint32_t* resume_tick);
+/* out = {members paused now, resumed Alive (the pause went unnoticed), resumed Suspect (a false suspicion,
+ * refuted), resumed Dead (declared Failed, now back)}. */
+int gsim_pause_stats(gsim_pool* p, uint64_t out[4]);
+
 /* ---- time ---------------------------------------------------------------- */
 int gsim_step(gsim_pool* p, uint32_t ticks);
 #define GSIM_PRED_RUMOR_CONVERGED 1 /* arg = slot: every UP member heard it          */
