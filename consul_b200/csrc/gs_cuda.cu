@@ -1207,6 +1207,13 @@ class CudaBackend : public GsBackend {
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&wocc, gs_window_kernel<false, false>, GS_BLOCK, 0) != cudaSuccess || wocc < 1)
       wocc = GS_WIN_BLOCKS;
     win_grid_ = (uint32_t)(sms * wocc);
+    // GSIM_GRID_MAX=<CTAs>: fewer CTAs for the tick and window kernels (their partitions depend on gridDim
+    // only), so that a pool small enough for the oracle to follow runs several rounds and batches per warp
+    if (const char* e = getenv("GSIM_GRID_MAX")) {
+      const long cap = atol(e);
+      if (cap > 0 && (unsigned long)cap < full_grid_) full_grid_ = (uint32_t)cap;
+      if (cap > 0 && (unsigned long)cap < win_grid_) win_grid_ = (uint32_t)cap;
+    }
     scratch_ = nullptr;
     cudaMalloc(&scratch_, 4096);
   }
