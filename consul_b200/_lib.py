@@ -125,6 +125,13 @@ SIGNATURES = [
     ("gsim_graph_set", _i32, [_P, _u32, C.POINTER(_u32), C.POINTER(_u32)]),
     ("gsim_member_reconnect_timeout_set", _i32, [_P, _u32, _u64]),
     ("gsim_coordinate_get", _i32, [_P, _u32, C.POINTER(C.c_double)]),
+    ("gsim_coordinates_read", _i32, [_P, _u32, _u32, C.POINTER(C.c_double)]),
+    ("gsim_rtt_many", _i32, [_P, C.POINTER(_u32), C.POINTER(_u32), _sz, C.POINTER(C.c_double),
+                             C.POINTER(C.c_double)]),
+    ("gsim_sort_by_distance", _i32, [_P, _u32, C.POINTER(_u32), _sz, _sz, C.POINTER(_u32),
+                                     C.POINTER(C.c_double)]),
+    ("gsim_dcs_by_distance", _i32, [_P, _u32, C.POINTER(_u32), _sz, C.POINTER(_u32), C.POINTER(C.c_double)]),
+    ("gsim_coordinate_error", _i32, [_P, _u32, _u32, C.POINTER(C.c_double)]),
     ("gsim_member_watch", _i32, [_P, _u32, _i32]),
     ("gsim_member_update", _i32, [_P, _u32, _u32, C.POINTER(_u32)]),
     ("gsim_step", _i32, [_P, _u32]),

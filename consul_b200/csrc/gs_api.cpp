@@ -25,6 +25,7 @@
 #include "gs_backend.h"
 #include "gs_wire.h"
 #include "gs_coord.h"
+#include "gs_query.h"
 
 #ifndef GS_MAKE_BACKEND
 #define GS_MAKE_BACKEND gs_make_cuda_backend
@@ -302,6 +303,11 @@ struct gsim_pool {
   uint32_t* pause_until = nullptr;
   uint64_t* pause_cnt_dev = nullptr;
   uint64_t pause_cnt[4] = {0, 0, 0, 0};
+  // network-coordinate queries (gsim_coordinates_read ...): (key, value) pairs for `capacity` entries and
+  // room for partial sums and small results, allocated by the first query that needs them
+  uint64_t* q_key = nullptr;
+  uint32_t* q_val = nullptr;
+  double* q_aux = nullptr;
   // host writes to device state not yet handed to the backend (see dev()), and whether handing an
   // earlier batch over failed (reported by the API call it belonged to)
   GsWriteBatch wb = {};
@@ -1639,6 +1645,326 @@ extern "C" int gsim_coordinate_get(gsim_pool* p, uint32_t id, double out[11]) {
   const size_t slot = tb > ta ? 1 : 0;
   for (size_t x = 0; x < GS_COORD_WORDS; ++x)
     if (!peek(p, p->d.coord, (slot * GS_COORD_WORDS + x) * cap + id, &out[x])) return fail(p, GSIM_ERR_CUDA, "peek");
+  return GSIM_OK;
+}
+
+// ---- network-coordinate queries (DESIGN.md §3.4 "Queries", gs_query.h) -----------------------------
+// The backend defaults (gs_backend.h): the coordinate columns copied to the host behind a GsDev of host
+// pointers, the query bodies of gs_query.h run there, the results copied back.
+namespace {
+struct HostCoords {
+  std::vector<double> coord;
+  std::vector<uint32_t> ctag, key;
+  std::vector<uint8_t> delay;
+  GsDev d;
+  bool load(GsBackend* be, const GsDev& dd, const GsGlobals& g, uint32_t now, bool keys) {
+    const size_t cap = g.cap;
+    d = dd;
+    coord.resize(cap * 2 * GS_COORD_WORDS);
+    ctag.resize(cap * 2);
+    if (!be->d2h(coord.data(), dd.coord, coord.size() * 8) || !be->d2h(ctag.data(), dd.ctag, ctag.size() * 4))
+      return false;
+    d.coord = coord.data();
+    d.ctag = ctag.data();
+    if (dd.imp_delay) {
+      delay.resize(cap);
+      if (!be->d2h(delay.data(), dd.imp_delay, cap)) return false;
+      d.imp_delay = delay.data();
+    }
+    if (keys) {
+      key.resize(g.n);
+      if (g.n && !be->d2h(key.data(), dd.key[now & 1u], (size_t)g.n * 4)) return false;
+      d.key[now & 1u] = key.data();
+    }
+    return true;
+  }
+};
+}  // namespace
+
+static_assert(sizeof(GsCoord) == GS_COORD_WORDS * sizeof(double), "a coordinate row is its 11 doubles");
+
+bool GsBackend::coord_rows(const GsDev& d, const GsGlobals& g, uint32_t first, uint32_t count, double* rows) {
+  if (!count) return true;
+  HostCoords h;
+  if (!h.load(this, d, g, 0u, false)) return false;
+  std::vector<GsCoord> out(count);
+  for (uint32_t x = 0; x < count; ++x) gs_coord_pick(h.d.coord, h.d.ctag, g.cap, first + x, out[x]);
+  return h2d(rows, out.data(), out.size() * sizeof(GsCoord));
+}
+
+bool GsBackend::coord_pairs(const GsDev& d, const GsGlobals*, const GsGlobals& g, const uint32_t* a, const uint32_t* b,
+                            uint32_t n, double* est, double* tru) {
+  if (!n) return true;
+  HostCoords h;
+  std::vector<uint32_t> ha(n), hb(n);
+  std::vector<double> he(n), ht(n);
+  if (!h.load(this, d, g, 0u, false) || !d2h(ha.data(), a, (size_t)n * 4) || !d2h(hb.data(), b, (size_t)n * 4))
+    return false;
+  for (uint32_t k = 0; k < n; ++k) {
+    GsCoord ca, cb;
+    gs_coord_pick(h.d.coord, h.d.ctag, g.cap, ha[k], ca);
+    gs_coord_pick(h.d.coord, h.d.ctag, g.cap, hb[k], cb);
+    he[k] = gs_coord_distance_seconds(ca, cb);
+    ht[k] = gs_model_rtt(g, h.d.imp_delay, ha[k], hb[k]);
+  }
+  return h2d(est, he.data(), (size_t)n * 8) && (!tru || h2d(tru, ht.data(), (size_t)n * 8));
+}
+
+bool GsBackend::coord_dist_from(const GsDev& d, const GsGlobals*, const GsGlobals& g, uint32_t now, uint32_t from,
+                                const uint32_t* ids, uint32_t n, bool router, uint64_t* key, uint32_t* val) {
+  if (!n) return true;
+  HostCoords h;
+  std::vector<uint32_t> hi(n);
+  std::vector<uint64_t> hk(n);
+  if (!h.load(this, d, g, now, router) || (ids && !d2h(hi.data(), ids, (size_t)n * 4))) return false;
+  GsCoord cf;
+  gs_coord_pick(h.d.coord, h.d.ctag, g.cap, from, cf);
+  for (uint32_t x = 0; x < n; ++x) {
+    const uint32_t s = ids ? hi[x] : x;
+    if (router) {
+      gs_router_entry(h.d, g, now, from, cf, s, &hk[x], &hi[x]);
+    } else {
+      GsCoord c;
+      gs_coord_pick(h.d.coord, h.d.ctag, g.cap, s, c);
+      hk[x] = gs_dist_key(gs_coord_distance_seconds(cf, c));
+      hi[x] = s;
+    }
+  }
+  return h2d(key, hk.data(), (size_t)n * 8) && h2d(val, hi.data(), (size_t)n * 4);
+}
+
+bool GsBackend::sort_pairs(const GsGlobals&, uint64_t* key, uint32_t* val, uint32_t n, uint32_t n_dcs) {
+  if (n < 2u) return true;
+  std::vector<uint64_t> hk(n), sk(n);
+  std::vector<uint32_t> hv(n), sv(n), ord(n);
+  if (!d2h(hk.data(), key, (size_t)n * 8) || !d2h(hv.data(), val, (size_t)n * 4)) return false;
+  for (uint32_t x = 0; x < n; ++x) ord[x] = x;
+  std::stable_sort(ord.begin(), ord.end(), [&](uint32_t a, uint32_t b) {
+    if (n_dcs) {
+      const uint32_t da = gs_dc_digit(hv[a], n_dcs), db = gs_dc_digit(hv[b], n_dcs);
+      if (da != db) return da < db;
+    }
+    return hk[a] < hk[b];
+  });
+  for (uint32_t x = 0; x < n; ++x) {
+    sk[x] = hk[ord[x]];
+    sv[x] = hv[ord[x]];
+  }
+  return h2d(key, sk.data(), (size_t)n * 8) && h2d(val, sv.data(), (size_t)n * 4);
+}
+
+bool GsBackend::dc_medians(const GsGlobals&, const uint64_t* key, const uint32_t* val, uint32_t n, uint32_t n_dcs,
+                           double* med, uint32_t* cnt) {
+  std::vector<uint64_t> hk(n);
+  std::vector<uint32_t> hv(n), hc(n_dcs, 0u), first(n_dcs, 0u);
+  std::vector<double> hm(n_dcs);
+  if (n && (!d2h(hk.data(), key, (size_t)n * 8) || !d2h(hv.data(), val, (size_t)n * 4))) return false;
+  for (uint32_t x = 0; x < n; ++x) {
+    const uint32_t c = gs_dc_digit(hv[x], n_dcs);
+    if (c >= n_dcs) continue;
+    if (!hc[c]) first[c] = x;
+    hc[c]++;
+  }
+  for (uint32_t c = 0; c < n_dcs; ++c) hm[c] = hc[c] ? gs_key_dist(hk[first[c] + hc[c] / 2u]) : gs_key_dist(0x7FF0000000000000ull);
+  return h2d(med, hm.data(), (size_t)n_dcs * 8) && h2d(cnt, hc.data(), (size_t)n_dcs * 4);
+}
+
+bool GsBackend::coord_error(const GsDev& d, const GsGlobals* g_dev, const GsGlobals& g, uint32_t now, uint32_t n_draws,
+                            uint32_t salt, uint64_t* key, uint32_t* val, double* part, double* out) {
+  const uint32_t nch = (n_draws + GS_ERR_CHUNK - 1u) / GS_ERR_CHUNK;
+  HostCoords h;
+  if (!h.load(this, d, g, now, true)) return false;
+  std::vector<uint64_t> hk(n_draws);
+  std::vector<uint32_t> hv(n_draws);
+  std::vector<double> hp(2 * (size_t)nch, 0.0);
+  for (uint32_t k = 0; k < n_draws; ++k) {
+    const double e = gs_error_draw(h.d, g, now, k, salt);
+    hv[k] = k;
+    hk[k] = ~0ull;
+    if (e < 0.0) continue;
+    hk[k] = gs_dist_key(e);
+    hp[k / GS_ERR_CHUNK] = hp[k / GS_ERR_CHUNK] + e;
+    hp[nch + k / GS_ERR_CHUNK] += 1.0;
+  }
+  if (!h2d(key, hk.data(), (size_t)n_draws * 8) || !h2d(val, hv.data(), (size_t)n_draws * 4) ||
+      !sort_pairs(g, key, val, n_draws, 0u) || !d2h(hk.data(), key, (size_t)n_draws * 8))
+    return false;
+  double ho[6];
+  gs_error_finish(hk.data(), n_draws, hp.data(), ho);
+  (void)g_dev;
+  return h2d(part, hp.data(), hp.size() * 8) && h2d(out, ho, sizeof(ho));
+}
+
+static int coord_query_check(gsim_pool* p) {
+  if (!p->d.coord) return fail(p, GSIM_ERR_STATE, "the pool was created without GSIM_FLAG_COORDINATES");
+  return GSIM_OK;
+}
+
+// q_aux: chunk sums and counts of gsim_coordinate_error (2 per GS_ERR_CHUNK draws of `capacity`), then
+// room for the small results (its 6 statistics; the per-datacenter medians and counts)
+static size_t query_aux_small(const gsim_pool* p) { return 2 * ((size_t)p->g.cap / GS_ERR_CHUNK + 1); }
+
+static bool query_alloc(gsim_pool* p) {
+  if (p->q_key) return true;
+  const size_t cap = p->g.cap;
+  uint64_t* k = nullptr;
+  uint32_t* v = nullptr;
+  double* a = nullptr;
+  if (!alloc_col(p, &k, cap) || !alloc_col(p, &v, cap) || !alloc_col(p, &a, query_aux_small(p) + 2 * GS_MAX_DCS))
+    return false;
+  p->q_key = k;
+  p->q_val = v;
+  p->q_aux = a;
+  return true;
+}
+
+static int check_ids(gsim_pool* p, const uint32_t* ids, size_t n) {
+  for (size_t x = 0; x < n; ++x)
+    if (ids[x] >= p->g.n) return fail(p, GSIM_ERR_NOT_FOUND, "unknown member");
+  return GSIM_OK;
+}
+
+// (*Serf).GetCoordinate for members [first, first + count) — what `consul rtt` and the catalog's
+// Coordinate.ListNodes read (agent/consul/coordinate_endpoint.go): out[11 x ..] is exactly what
+// gsim_coordinate_get returns for member first + x.
+extern "C" int gsim_coordinates_read(gsim_pool* p, uint32_t first, uint32_t count, double* out) {
+  if (!p || (!out && count)) return GSIM_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(p->mu);
+  GS_CONTROLLER_ONLY(p);
+  int rc = coord_query_check(p);
+  if (rc) return rc;
+  if (first > p->g.n || count > p->g.n - first) return fail(p, GSIM_ERR_NOT_FOUND, "unknown member");
+  if (!count) return GSIM_OK;
+  const size_t bytes = (size_t)count * sizeof(GsCoord);
+  double* rows = reinterpret_cast<double*>(dev(p)->alloc(bytes));
+  if (!rows) return fail(p, GSIM_ERR_NOMEM, "coordinate rows");
+  const bool okk = dev(p)->coord_rows(p->d, p->g, first, count, rows) && dev(p)->d2h(out, rows, bytes);
+  dev(p)->release(rows);
+  return okk ? GSIM_OK : fail(p, GSIM_ERR_CUDA, "coord_rows");
+}
+
+// librtt.ComputeDistance (internal/gossip/librtt/rtt.go:16-22), what `consul rtt` prints, for n pairs; and the
+// round trip a direct probe between them samples in the model (§3.5), to measure the embedding against.
+extern "C" int gsim_rtt_many(gsim_pool* p, const uint32_t* a, const uint32_t* b, size_t n, double* est_s,
+                             double* true_s) {
+  if (!p || (n && (!a || !b || !est_s)) || n > 0x7FFFFFFFu) return GSIM_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(p->mu);
+  GS_CONTROLLER_ONLY(p);
+  int rc = coord_query_check(p);
+  if (!rc) rc = check_ids(p, a, n);
+  if (!rc) rc = check_ids(p, b, n);
+  if (rc || !n) return rc;
+  if (!upload_globals(p)) return fail(p, GSIM_ERR_CUDA, "upload");
+  // one buffer: a, b, then the estimates and the true round trips next to each other (one readback)
+  uint8_t* buf = reinterpret_cast<uint8_t*>(dev(p)->alloc(n * 24));
+  if (!buf) return fail(p, GSIM_ERR_NOMEM, "pair buffers");
+  uint32_t* da = reinterpret_cast<uint32_t*>(buf);
+  uint32_t* db = da + n;
+  double* de = reinterpret_cast<double*>(buf + n * 8);
+  double* dt = true_s ? de + n : nullptr;
+  std::vector<double> back(true_s ? 2 * n : 0);
+  bool okk = dev(p)->h2d_async(da, a, n * 4) && dev(p)->h2d_async(db, b, n * 4) &&
+             dev(p)->coord_pairs(p->d, p->g_dev, p->g, da, db, (uint32_t)n, de, dt);
+  if (okk && true_s) {
+    okk = dev(p)->d2h(back.data(), de, n * 16);
+    if (okk) {
+      memcpy(est_s, back.data(), n * 8);
+      memcpy(true_s, back.data() + n, n * 8);
+    }
+  } else if (okk) {
+    okk = dev(p)->d2h(est_s, de, n * 8);
+  }
+  dev(p)->release(buf);
+  return okk ? GSIM_OK : fail(p, GSIM_ERR_CUDA, "coord_pairs");
+}
+
+// sortNodesByDistanceFrom (agent/consul/rtt.go:14-52, 190-220): the ?near= order of catalog and health results,
+// a sort.Stable of `ids` (NULL: every created member, in id order) by ComputeDistance from `from`.  The first k
+// results are written (k = n for the whole order, small k for NearestN); ties keep input order.
+extern "C" int gsim_sort_by_distance(gsim_pool* p, uint32_t from, const uint32_t* ids, size_t n, size_t k,
+                                     uint32_t* out_ids, double* out_dist) {
+  if (!p) return GSIM_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(p->mu);
+  GS_CONTROLLER_ONLY(p);
+  int rc = coord_query_check(p);
+  if (rc) return rc;
+  const size_t count = ids ? n : p->g.n;
+  if (from >= p->g.n) return fail(p, GSIM_ERR_NOT_FOUND, "unknown member");
+  if (ids && (rc = check_ids(p, ids, n))) return rc;
+  if (count > p->g.cap) return fail(p, GSIM_ERR_INVALID, "more ids than the pool's capacity");
+  if (k > count || (k && !out_ids)) return fail(p, GSIM_ERR_INVALID, "k must be <= the number of ids");
+  if (!count) return GSIM_OK;
+  if (!query_alloc(p)) return fail(p, GSIM_ERR_NOMEM, "query buffers");
+  if (!upload_globals(p)) return fail(p, GSIM_ERR_CUDA, "upload");
+  GsBackend* be = dev(p);
+  bool okk = (!ids || be->h2d_async(p->q_val, ids, count * 4)) &&
+             be->coord_dist_from(p->d, p->g_dev, p->g, p->now, from, ids ? p->q_val : nullptr, (uint32_t)count, false,
+                                 p->q_key, p->q_val) &&
+             be->sort_pairs(p->g, p->q_key, p->q_val, (uint32_t)count, 0u);
+  if (okk && k) okk = be->d2h(out_ids, p->q_val, k * 4) && (!out_dist || be->d2h(out_dist, p->q_key, k * 8));
+  if (okk && !k) okk = be->sync();
+  return okk ? GSIM_OK : fail(p, GSIM_ERR_CUDA, "sort_by_distance");
+}
+
+// Router.GetDatacentersByDistance (agent/router/router.go:537-615) for one area, seen from `from`: every server
+// (servers == NULL: every member, as in a WAN pool) that the view does not list Left and that still exists
+// counts, in datacenter (i / 128) % n_dcs; one in from's own datacenter at 0.0, every other at ComputeDistance.
+// A datacenter's RTT is rtts[len / 2] of its sorted RTTs; datacenters are stable-sorted by it, ties in index
+// order (where upstream's sort.Strings pass over DC names stands).  dc_order / dc_rtt hold n_dcs entries; a
+// datacenter without a counted server (upstream: absent) comes last with dc_rtt = +inf.
+extern "C" int gsim_dcs_by_distance(gsim_pool* p, uint32_t from, const uint32_t* servers, size_t n_servers,
+                                    uint32_t* dc_order, double* dc_rtt) {
+  if (!p || !dc_order || !dc_rtt || (!servers && n_servers)) return GSIM_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(p->mu);
+  GS_CONTROLLER_ONLY(p);
+  int rc = coord_query_check(p);
+  if (rc) return rc;
+  const uint32_t n_dcs = p->g.n_dcs;
+  if (!n_dcs) return fail(p, GSIM_ERR_STATE, "the pool has no latency matrix (no datacenters)");
+  if (from >= p->g.n) return fail(p, GSIM_ERR_NOT_FOUND, "unknown member");
+  if (servers && (rc = check_ids(p, servers, n_servers))) return rc;
+  const size_t count = servers ? n_servers : p->g.n;
+  if (count > p->g.cap) return fail(p, GSIM_ERR_INVALID, "more servers than the pool's capacity");
+  if (!query_alloc(p)) return fail(p, GSIM_ERR_NOMEM, "query buffers");
+  if (!upload_globals(p)) return fail(p, GSIM_ERR_CUDA, "upload");
+  GsBackend* be = dev(p);
+  double* med = p->q_aux;
+  uint32_t* cnt = reinterpret_cast<uint32_t*>(p->q_aux + GS_MAX_DCS);
+  double m[GS_MAX_DCS];
+  const bool okk = (!servers || be->h2d_async(p->q_val, servers, count * 4)) &&
+                   be->coord_dist_from(p->d, p->g_dev, p->g, p->now, from, servers ? p->q_val : nullptr, (uint32_t)count,
+                                       true, p->q_key, p->q_val) &&
+                   be->sort_pairs(p->g, p->q_key, p->q_val, (uint32_t)count, n_dcs) &&
+                   be->dc_medians(p->g, p->q_key, p->q_val, (uint32_t)count, n_dcs, med, cnt) &&
+                   be->d2h(m, med, (size_t)n_dcs * 8);
+  if (!okk) return fail(p, GSIM_ERR_CUDA, "dcs_by_distance");
+  uint32_t ord[GS_MAX_DCS];
+  for (uint32_t c = 0; c < n_dcs; ++c) ord[c] = c;
+  std::stable_sort(ord, ord + n_dcs, [&](uint32_t a, uint32_t b) { return m[a] < m[b]; });
+  for (uint32_t c = 0; c < n_dcs; ++c) {
+    dc_order[c] = ord[c];
+    dc_rtt[c] = m[ord[c]];
+  }
+  return GSIM_OK;
+}
+
+// How well the embedding predicts the model's round trips (SURVEY §8f N3): over the draws k < n_draws of
+// philox(seed; k, salt, GS_PUR_COORD_SAMPLE) = (x, y, ..), the pairs (x mod n, y mod n) of two different running
+// members; out = {pairs kept, mean, p50, p90, p99, max} of |ComputeDistance - true| / true (gs_query.h).
+extern "C" int gsim_coordinate_error(gsim_pool* p, uint32_t n_draws, uint32_t salt, double out[6]) {
+  if (!p || !out) return GSIM_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(p->mu);
+  GS_CONTROLLER_ONLY(p);
+  int rc = coord_query_check(p);
+  if (rc) return rc;
+  if (n_draws == 0u || n_draws > p->g.cap) return fail(p, GSIM_ERR_INVALID, "n_draws must be in [1, capacity]");
+  if (!p->g.n) return fail(p, GSIM_ERR_STATE, "the pool has no members");
+  if (!query_alloc(p)) return fail(p, GSIM_ERR_NOMEM, "query buffers");
+  if (!upload_globals(p)) return fail(p, GSIM_ERR_CUDA, "upload");
+  double* dout = p->q_aux + query_aux_small(p);
+  if (!dev(p)->coord_error(p->d, p->g_dev, p->g, p->now, n_draws, salt, p->q_key, p->q_val, p->q_aux, dout) ||
+      !dev(p)->d2h(out, dout, 6 * sizeof(double)))
+    return fail(p, GSIM_ERR_CUDA, "coordinate_error");
   return GSIM_OK;
 }
 

@@ -235,6 +235,31 @@ class GsBackend {
                           uint32_t* n_paused);
   virtual bool resume_rows(const GsDev& d, const GsGlobals* g_dev, const GsGlobals& g, uint32_t* pause_until,
                            uint32_t t, bool resume, bool log_events, uint32_t counts[4]);
+  // ---- network-coordinate queries (gs_query.h, DESIGN.md §3.4 "Queries"; single-GPU pools) ----------
+  // Read-only.  Every pointer is device memory and nothing is waited for: the caller reads the result
+  // back once.  Defined in gs_api.cpp through the copy primitives every backend has, which is what the
+  // host emulation runs; the CUDA backend replaces each with sm_90a kernels.
+  // rows[11 x ..] = the published coordinate (gs_coord_pick) of member first + x
+  virtual bool coord_rows(const GsDev& d, const GsGlobals& g, uint32_t first, uint32_t count, double* rows);
+  // est[k] = the distance between a[k] and b[k]; tru[k] (tru may be null) = gs_model_rtt(a[k], b[k])
+  virtual bool coord_pairs(const GsDev& d, const GsGlobals* g_dev, const GsGlobals& g, const uint32_t* a,
+                           const uint32_t* b, uint32_t n, double* est, double* tru);
+  // key[x] = gs_dist_key of the distance from `from` to ids[x] (ids null: to member x), val[x] = that id; or
+  // (router) gs_router_entry at tick now.  ids may be val.
+  virtual bool coord_dist_from(const GsDev& d, const GsGlobals* g_dev, const GsGlobals& g, uint32_t now, uint32_t from,
+                               const uint32_t* ids, uint32_t n, bool router, uint64_t* key, uint32_t* val);
+  // stable sort of the n pairs (key[x], val[x]) by key, or (n_dcs != 0) by (gs_dc_digit(val), key)
+  virtual bool sort_pairs(const GsGlobals& g, uint64_t* key, uint32_t* val, uint32_t n, uint32_t n_dcs);
+  // over pairs sorted by (datacenter, key): cnt[c] = entries of datacenter c < n_dcs, med[c] = the distance of
+  // its entry cnt[c] / 2 (+inf when it has none)
+  virtual bool dc_medians(const GsGlobals& g, const uint64_t* key, const uint32_t* val, uint32_t n, uint32_t n_dcs,
+                          double* med, uint32_t* cnt);
+  // gsim_coordinate_error: draws [0, n_draws) at tick now into key (gs_dist_key of the relative error, all ones
+  // when skipped) and val (the draw), sorted by sort_pairs; then out = {kept, mean, p50, p90, p99, max}, the
+  // mean = (sum over chunks of GS_ERR_CHUNK draws, in chunk order, of the chunk's errors summed in draw order) /
+  // kept.  `part` has room for 2 ceil(n_draws / GS_ERR_CHUNK) doubles.
+  virtual bool coord_error(const GsDev& d, const GsGlobals* g_dev, const GsGlobals& g, uint32_t now, uint32_t n_draws,
+                           uint32_t salt, uint64_t* key, uint32_t* val, double* part, double* out);
   // counts over members [first, first + count) (a rank of a sharded pool counts its own rows)
   virtual bool recount(const GsDev& d, const GsGlobals* g_dev, const GsGlobals& g, uint32_t now, uint32_t first,
                        uint32_t count, GsRecount* out) = 0;

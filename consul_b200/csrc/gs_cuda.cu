@@ -9,6 +9,8 @@
 //   gs_stretch_*        drive a tick stretch: single ticks until the pool is quiet, decided on the device
 //   gs_init_kernel, gs_crash_kernel, gs_recount_kernel, gs_hash_kernel   control plane
 //   gs_pause_kernel, gs_resume_kernel   paused members (gsim_pause_*, DESIGN.md §3.6)
+//   gs_coord_*_kernel, gs_rs_*_kernel   network-coordinate queries and their stable LSD radix sort
+//                                       (DESIGN.md §3.4 "Queries")
 //
 // Launch shape of the tick: a persistent grid (SMs x resident CTAs) of 256-thread CTAs; every warp
 // owns a contiguous chunk of 128-member tiles, scans their 4-byte mailbox words through a
@@ -24,6 +26,7 @@
 
 #include "gs_aux.h"
 #include "gs_backend.h"
+#include "gs_query.h"
 #include "gs_vmm.h"
 
 #define GS_BLOCK 256
@@ -1190,6 +1193,284 @@ __global__ void __launch_bounds__(GS_BLOCK) gs_and_kernel(GsDev d, uint32_t firs
   }
 }
 
+// ---- network-coordinate queries (gs_query.h, DESIGN.md §3.4 "Queries") ------------------------------
+// Rows of 11 doubles for GS_BLOCK members per CTA: each member's published slot is read coalesced over the
+// SoA planes into shared memory, then the CTA writes its rows out contiguously.
+__global__ void __launch_bounds__(GS_BLOCK)
+    gs_coord_rows_kernel(GsDev d, uint32_t cap, uint32_t first, uint32_t count, double* rows) {
+  __shared__ GsCoord s[GS_BLOCK];
+  const uint32_t x0 = blockIdx.x * GS_BLOCK;
+  const uint32_t m = count - x0 < GS_BLOCK ? count - x0 : GS_BLOCK;
+  if (threadIdx.x < m) gs_coord_pick(d.coord, d.ctag, cap, first + x0 + threadIdx.x, s[threadIdx.x]);
+  __syncthreads();
+  const double* sw = reinterpret_cast<const double*>(s);
+  double* out = rows + (size_t)x0 * GS_COORD_WORDS;
+  for (uint32_t t = threadIdx.x; t < m * GS_COORD_WORDS; t += GS_BLOCK) out[t] = sw[t];
+}
+
+__global__ void __launch_bounds__(GS_BLOCK)
+    gs_coord_pairs_kernel(GsDev d, const GsGlobals* __restrict__ gp, const uint32_t* a, const uint32_t* b, uint32_t n,
+                          double* est, double* tru) {
+  const uint32_t k = blockIdx.x * GS_BLOCK + threadIdx.x;
+  if (k >= n) return;
+  const GsGlobals& g = *gp;
+  const uint32_t i = a[k], j = b[k];
+  GsCoord ci, cj;
+  gs_coord_pick(d.coord, d.ctag, g.cap, i, ci);
+  gs_coord_pick(d.coord, d.ctag, g.cap, j, cj);
+  est[k] = gs_coord_distance_seconds(ci, cj);
+  if (tru != nullptr) tru[k] = gs_model_rtt(g, d.imp_delay, i, j);
+}
+
+__global__ void __launch_bounds__(GS_BLOCK)
+    gs_coord_dist_kernel(GsDev d, const GsGlobals* __restrict__ gp, uint32_t now, uint32_t from, const uint32_t* ids,
+                         uint32_t n, uint32_t router, uint64_t* key, uint32_t* val) {
+  const uint32_t x = blockIdx.x * GS_BLOCK + threadIdx.x;
+  if (x >= n) return;
+  const GsGlobals& g = *gp;
+  GsCoord cf;
+  gs_coord_pick(d.coord, d.ctag, g.cap, from, cf);  // (the same 11 words for every thread: L1 broadcasts)
+  const uint32_t s = ids != nullptr ? ids[x] : x;
+  uint64_t k;
+  uint32_t v = s;
+  if (router) {
+    gs_router_entry(d, g, now, from, cf, s, &k, &v);
+  } else {
+    GsCoord c;
+    gs_coord_pick(d.coord, d.ctag, g.cap, s, c);
+    k = gs_dist_key(gs_coord_distance_seconds(cf, c));
+  }
+  // device assertion: the radix sort orders these bits as unsigned integers, which is the order of the
+  // distances only for finite values with the sign clear (__trap, not assert: no host-call machinery)
+  if (v != GS_EMPTY32 && !gs_dist_key_ok(k)) __trap();
+  key[x] = k;
+  val[x] = v;
+}
+
+// Chunk c of gsim_coordinate_error's draws is CTA c: every thread takes one draw, thread 0 adds the kept
+// errors in draw order.
+__global__ void __launch_bounds__(GS_BLOCK)
+    gs_coord_error_kernel(GsDev d, const GsGlobals* __restrict__ gp, uint32_t now, uint32_t n_draws, uint32_t salt,
+                          uint64_t* key, uint32_t* val, double* part) {
+  static_assert(GS_ERR_CHUNK == GS_BLOCK, "one CTA per chunk of draws");
+  __shared__ double s[GS_BLOCK];
+  const uint32_t k = blockIdx.x * GS_BLOCK + threadIdx.x;
+  double e = -1.0;
+  if (k < n_draws) {
+    e = gs_error_draw(d, *gp, now, k, salt);
+    const uint64_t bits = e < 0.0 ? ~0ull : gs_dist_key(e);
+    if (e >= 0.0 && !gs_dist_key_ok(bits)) __trap();  // device assertion, as in gs_coord_dist_kernel
+    key[k] = bits;
+    val[k] = k;
+  }
+  s[threadIdx.x] = e;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double sum = 0.0, kept = 0.0;
+    for (uint32_t x = 0; x < GS_BLOCK; ++x)
+      if (s[x] >= 0.0) {
+        sum = sum + s[x];
+        kept += 1.0;
+      }
+    part[blockIdx.x] = sum;
+    part[gridDim.x + blockIdx.x] = kept;
+  }
+}
+
+__global__ void gs_coord_error_finish_kernel(const uint64_t* sorted, uint32_t n_draws, const double* part, double* out) {
+  gs_error_finish(sorted, n_draws, part, out);
+}
+
+// Per-datacenter medians over pairs sorted by (gs_dc_digit, key): thread c finds datacenter c's run by binary
+// search.
+__global__ void gs_dc_medians_kernel(const uint64_t* key, const uint32_t* val, uint32_t n, uint32_t n_dcs, double* med,
+                                     uint32_t* cnt) {
+  const uint32_t c = threadIdx.x;
+  if (c >= n_dcs) return;
+  uint32_t lo = 0, hi = n;  // first entry with digit >= c
+  while (lo < hi) {
+    const uint32_t mid = lo + (hi - lo) / 2u;
+    if (gs_dc_digit(val[mid], n_dcs) < c) lo = mid + 1u; else hi = mid;
+  }
+  uint32_t end = lo, top = n;  // first entry with digit > c
+  while (end < top) {
+    const uint32_t mid = end + (top - end) / 2u;
+    if (gs_dc_digit(val[mid], n_dcs) <= c) end = mid + 1u; else top = mid;
+  }
+  cnt[c] = end - lo;
+  med[c] = end > lo ? gs_key_dist(key[lo + (end - lo) / 2u]) : gs_key_dist(0x7FF0000000000000ull);
+}
+
+// ---- stable LSD radix sort of (u64 key, u32 value) pairs ---------------------------------------------
+// 8-bit digits: passes 0..7 over the key from the least significant byte, then (by datacenter) pass 8 over
+// gs_dc_digit(value).  Per pass: an upsweep histogram per tile of GS_RS_TILE pairs, an exclusive scan of every
+// digit's counts over the tiles, and a scatter that ranks each tile's pairs stably (warp match + per-warp
+// digit counts, rounds of GS_BLOCK pairs in input order).  One histogram of every pass up front lets the
+// device skip a pass whose digit is the same for every pair; which buffer each pass reads is decided there too.
+#define GS_RS_TILE 4096u
+#define GS_RS_PASSES 9u
+struct GsRsCtl {
+  uint32_t skip[GS_RS_PASSES];
+  uint32_t src[GS_RS_PASSES];  // buffer (0 = the caller's, 1 = the backend's) pass p reads
+  uint32_t fin;                // buffer holding the result
+};
+struct GsRsBufs {
+  uint64_t* key[2];
+  uint32_t* val[2];
+};
+
+__device__ __forceinline__ uint32_t gs_rs_digit(uint64_t k, uint32_t v, uint32_t p, uint32_t n_dcs) {
+  return p < 8u ? (uint32_t)(k >> (8u * p)) & 255u : gs_dc_digit(v, n_dcs);
+}
+
+__global__ void __launch_bounds__(GS_BLOCK)
+    gs_rs_hist_kernel(const uint64_t* key, const uint32_t* val, uint32_t n, uint32_t n_dcs, uint32_t np, uint32_t* ghist) {
+  __shared__ uint32_t s[GS_RS_PASSES * 256];
+  for (uint32_t x = threadIdx.x; x < np * 256u; x += GS_BLOCK) s[x] = 0u;
+  __syncthreads();
+  for (size_t x = (size_t)blockIdx.x * GS_BLOCK + threadIdx.x; x < n; x += (size_t)gridDim.x * GS_BLOCK) {
+    const uint64_t k = key[x];
+    const uint32_t v = np > 8u ? val[x] : 0u;
+    for (uint32_t p = 0; p < np; ++p) atomicAdd(&s[p * 256u + gs_rs_digit(k, v, p, n_dcs)], 1u);
+  }
+  __syncthreads();
+  for (uint32_t x = threadIdx.x; x < np * 256u; x += GS_BLOCK)
+    if (s[x]) atomicAdd(&ghist[x], s[x]);
+}
+
+__global__ void gs_rs_plan_kernel(const uint32_t* ghist, uint32_t n, uint32_t np, GsRsCtl* c) {
+  uint32_t src = 0u;
+  for (uint32_t p = 0; p < np; ++p) {
+    uint32_t top = 0u;
+    for (uint32_t dg = 0; dg < 256u; ++dg) top = ghist[p * 256u + dg] > top ? ghist[p * 256u + dg] : top;
+    c->skip[p] = top == n ? 1u : 0u;
+    c->src[p] = src;
+    if (top != n) src ^= 1u;
+  }
+  c->fin = src;
+}
+
+__global__ void __launch_bounds__(GS_BLOCK)
+    gs_rs_upsweep_kernel(GsRsBufs b, const GsRsCtl* c, uint32_t p, uint32_t n, uint32_t n_dcs, uint32_t* hist) {
+  if (c->skip[p]) return;
+  __shared__ uint32_t s[256];
+  s[threadIdx.x] = 0u;
+  __syncthreads();
+  const uint64_t* key = b.key[c->src[p]];
+  const uint32_t* val = b.val[c->src[p]];
+  const size_t t0 = (size_t)blockIdx.x * GS_RS_TILE, t1 = t0 + GS_RS_TILE < n ? t0 + GS_RS_TILE : n;
+  for (size_t x = t0 + threadIdx.x; x < t1; x += GS_BLOCK)
+    atomicAdd(&s[gs_rs_digit(key[x], p == 8u ? val[x] : 0u, p, n_dcs)], 1u);
+  __syncthreads();
+  hist[(size_t)threadIdx.x * gridDim.x + blockIdx.x] = s[threadIdx.x];
+}
+
+// Exclusive scan of GS_BLOCK values across the CTA; *total = their sum.
+__device__ __forceinline__ uint32_t gs_block_scan(uint32_t v, uint32_t* sw, uint32_t* total) {
+  const uint32_t lane = threadIdx.x & 31u, w = threadIdx.x >> 5;
+  uint32_t incl = v;
+  for (uint32_t o = 1; o < 32u; o <<= 1) {
+    const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, incl, o);
+    if (lane >= o) incl += y;
+  }
+  if (lane == 31u) sw[w] = incl;
+  __syncthreads();
+  if (w == 0) {
+    uint32_t t = lane < GS_WARPS ? sw[lane] : 0u, ti = t;
+    for (uint32_t o = 1; o < 32u; o <<= 1) {
+      const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, ti, o);
+      if (lane >= o) ti += y;
+    }
+    if (lane < GS_WARPS) sw[lane] = ti - t;
+    if (lane == GS_WARPS - 1u) sw[GS_WARPS] = ti;
+  }
+  __syncthreads();
+  const uint32_t r = sw[w] + incl - v;
+  *total = sw[GS_WARPS];
+  __syncthreads();
+  return r;
+}
+
+// CTA dg scans digit dg's counts over the nb tiles in place.
+__global__ void __launch_bounds__(GS_BLOCK) gs_rs_scan_kernel(const GsRsCtl* c, uint32_t p, uint32_t nb, uint32_t* hist) {
+  if (c->skip[p]) return;
+  __shared__ uint32_t sw[GS_WARPS + 1];
+  uint32_t* row = hist + (size_t)blockIdx.x * nb;
+  uint32_t carry = 0u;
+  for (uint32_t x0 = 0; x0 < nb; x0 += GS_BLOCK) {
+    const uint32_t x = x0 + threadIdx.x;
+    const uint32_t v = x < nb ? row[x] : 0u;
+    uint32_t total;
+    const uint32_t e = gs_block_scan(v, sw, &total);
+    if (x < nb) row[x] = carry + e;
+    carry += total;
+  }
+}
+
+__global__ void __launch_bounds__(GS_BLOCK)
+    gs_rs_scatter_kernel(GsRsBufs b, const GsRsCtl* c, uint32_t p, uint32_t n, uint32_t n_dcs, const uint32_t* hist,
+                         const uint32_t* ghist) {
+  if (c->skip[p]) return;
+  __shared__ uint32_t base[256];
+  __shared__ uint32_t wcnt[GS_WARPS][256];
+  __shared__ uint32_t woff[GS_WARPS][256];
+  __shared__ uint32_t sw[GS_WARPS + 1];
+  const uint32_t tid = threadIdx.x, lane = tid & 31u, w = tid >> 5;
+  // where this tile's pairs of digit tid start: pairs of smaller digits, then earlier tiles' of this digit
+  uint32_t total;
+  const uint32_t before = gs_block_scan(ghist[p * 256u + tid], sw, &total);
+  base[tid] = before + hist[(size_t)tid * gridDim.x + blockIdx.x];
+  for (uint32_t q = 0; q < GS_WARPS; ++q) wcnt[q][tid] = 0u;
+  __syncthreads();
+  const uint32_t s = c->src[p];
+  const uint64_t* ks = b.key[s];
+  const uint32_t* vs = b.val[s];
+  uint64_t* kd = b.key[s ^ 1u];
+  uint32_t* vd = b.val[s ^ 1u];
+  const size_t t0 = (size_t)blockIdx.x * GS_RS_TILE, t1 = t0 + GS_RS_TILE < n ? t0 + GS_RS_TILE : n;
+  const uint32_t lt = (1u << lane) - 1u;
+  for (size_t r0 = t0; r0 < t1; r0 += GS_BLOCK) {
+    const size_t x = r0 + tid;
+    const bool valid = x < t1;
+    uint64_t k = 0;
+    uint32_t v = 0, dg = 256u;  // (an out-of-range pair matches only its own kind)
+    if (valid) {
+      k = ks[x];
+      v = vs[x];
+      dg = gs_rs_digit(k, v, p, n_dcs);
+    }
+    const uint32_t peers = __match_any_sync(0xFFFFFFFFu, dg);
+    const uint32_t rank = __popc(peers & lt);
+    if (valid && rank == 0u) wcnt[w][dg] = __popc(peers);
+    __syncthreads();
+    {  // thread tid: digit tid's offsets per warp, in warp order
+      uint32_t acc = base[tid];
+      for (uint32_t q = 0; q < GS_WARPS; ++q) {
+        const uint32_t cq = wcnt[q][tid];
+        woff[q][tid] = acc;
+        acc += cq;
+        wcnt[q][tid] = 0u;
+      }
+      base[tid] = acc;
+    }
+    __syncthreads();
+    if (valid) {
+      const uint32_t pos = woff[w][dg] + rank;
+      kd[pos] = k;
+      vd[pos] = v;
+    }
+  }
+}
+
+// The result back into the caller's buffers when the last pass wrote the backend's.
+__global__ void __launch_bounds__(GS_BLOCK) gs_rs_copyback_kernel(GsRsBufs b, const GsRsCtl* c, uint32_t n) {
+  if (c->fin == 0u) return;
+  for (size_t x = (size_t)blockIdx.x * GS_BLOCK + threadIdx.x; x < n; x += (size_t)gridDim.x * GS_BLOCK) {
+    b.key[0][x] = b.key[1][x];
+    b.val[0][x] = b.val[1][x];
+  }
+}
+
 class CudaBackend : public GsBackend {
  public:
   explicit CudaBackend(int dev) : dev_(dev) {
@@ -1224,6 +1505,7 @@ class CudaBackend : public GsBackend {
     for (auto& kv : sgraphs_) cudaGraphExecDestroy(kv.second);
     if (sharded_) vmm_.destroy();
     if (scratch_) cudaFree(scratch_);
+    if (rs_mem_) cudaFree(rs_mem_);
     cudaEventDestroy(ev0_);
     cudaEventDestroy(ev1_);
     cudaStreamDestroy(stream_);
@@ -1565,6 +1847,73 @@ class CudaBackend : public GsBackend {
     }
     return ok(cudaGetLastError(), "resume launch") && d2h(counts, cnt, 16);
   }
+  // ---- network-coordinate queries: enqueued only, the caller reads back -----------------------------
+  bool coord_rows(const GsDev& d, const GsGlobals& g, uint32_t first, uint32_t count, double* rows) override {
+    cudaSetDevice(dev_);
+    if (!count) return true;
+    gs_coord_rows_kernel<<<(count + GS_BLOCK - 1) / GS_BLOCK, GS_BLOCK, 0, stream_>>>(d, g.cap, first, count, rows);
+    ++launches_;
+    return ok(cudaGetLastError(), "coordinate rows launch");
+  }
+  bool coord_pairs(const GsDev& d, const GsGlobals* g_dev, const GsGlobals&, const uint32_t* a, const uint32_t* b,
+                   uint32_t n, double* est, double* tru) override {
+    cudaSetDevice(dev_);
+    if (!n) return true;
+    gs_coord_pairs_kernel<<<(n + GS_BLOCK - 1) / GS_BLOCK, GS_BLOCK, 0, stream_>>>(d, g_dev, a, b, n, est, tru);
+    ++launches_;
+    return ok(cudaGetLastError(), "coordinate pairs launch");
+  }
+  bool coord_dist_from(const GsDev& d, const GsGlobals* g_dev, const GsGlobals&, uint32_t now, uint32_t from,
+                       const uint32_t* ids, uint32_t n, bool router, uint64_t* key, uint32_t* val) override {
+    cudaSetDevice(dev_);
+    if (!n) return true;
+    gs_coord_dist_kernel<<<(n + GS_BLOCK - 1) / GS_BLOCK, GS_BLOCK, 0, stream_>>>(d, g_dev, now, from, ids, n,
+                                                                                 router ? 1u : 0u, key, val);
+    ++launches_;
+    return ok(cudaGetLastError(), "coordinate distance launch");
+  }
+  bool sort_pairs(const GsGlobals& g, uint64_t* key, uint32_t* val, uint32_t n, uint32_t n_dcs) override {
+    cudaSetDevice(dev_);
+    if (n < 2u) return true;
+    if (!rs_reserve(g.cap > n ? g.cap : n)) return false;
+    const uint32_t np = n_dcs ? GS_RS_PASSES : 8u, nb = (n + GS_RS_TILE - 1u) / GS_RS_TILE;
+    uint32_t hb = nb < sms_ * 4u ? nb : sms_ * 4u;
+    if (!ok(cudaMemsetAsync(rs_ghist_, 0, GS_RS_PASSES * 256 * 4, stream_), "memset")) return false;
+    gs_rs_hist_kernel<<<hb, GS_BLOCK, 0, stream_>>>(key, val, n, n_dcs, np, rs_ghist_);
+    gs_rs_plan_kernel<<<1, 1, 0, stream_>>>(rs_ghist_, n, np, rs_ctl_);
+    GsRsBufs b;
+    b.key[0] = key;
+    b.key[1] = rs_key_;
+    b.val[0] = val;
+    b.val[1] = rs_val_;
+    for (uint32_t p = 0; p < np; ++p) {
+      gs_rs_upsweep_kernel<<<nb, GS_BLOCK, 0, stream_>>>(b, rs_ctl_, p, n, n_dcs, rs_hist_);
+      gs_rs_scan_kernel<<<256, GS_BLOCK, 0, stream_>>>(rs_ctl_, p, nb, rs_hist_);
+      gs_rs_scatter_kernel<<<nb, GS_BLOCK, 0, stream_>>>(b, rs_ctl_, p, n, n_dcs, rs_hist_, rs_ghist_);
+    }
+    hb = (n + GS_BLOCK - 1) / GS_BLOCK < sms_ * 8u ? (n + GS_BLOCK - 1) / GS_BLOCK : sms_ * 8u;
+    gs_rs_copyback_kernel<<<hb, GS_BLOCK, 0, stream_>>>(b, rs_ctl_, n);
+    launches_ += 3u + 3u * np;
+    return ok(cudaGetLastError(), "radix sort launch");
+  }
+  bool dc_medians(const GsGlobals&, const uint64_t* key, const uint32_t* val, uint32_t n, uint32_t n_dcs, double* med,
+                  uint32_t* cnt) override {
+    cudaSetDevice(dev_);
+    gs_dc_medians_kernel<<<1, GS_MAX_DCS, 0, stream_>>>(key, val, n, n_dcs, med, cnt);
+    ++launches_;
+    return ok(cudaGetLastError(), "medians launch");
+  }
+  bool coord_error(const GsDev& d, const GsGlobals* g_dev, const GsGlobals& g, uint32_t now, uint32_t n_draws,
+                   uint32_t salt, uint64_t* key, uint32_t* val, double* part, double* out) override {
+    cudaSetDevice(dev_);
+    const uint32_t nch = (n_draws + GS_ERR_CHUNK - 1u) / GS_ERR_CHUNK;
+    gs_coord_error_kernel<<<nch, GS_BLOCK, 0, stream_>>>(d, g_dev, now, n_draws, salt, key, val, part);
+    ++launches_;
+    if (!ok(cudaGetLastError(), "error sample launch") || !sort_pairs(g, key, val, n_draws, 0u)) return false;
+    gs_coord_error_finish_kernel<<<1, 1, 0, stream_>>>(key, n_draws, part, out);
+    ++launches_;
+    return ok(cudaGetLastError(), "error finish launch");
+  }
   bool reap_rows(const GsDev& d, const GsGlobals* g_dev, const GsGlobals& g, uint32_t now,
                  uint32_t reconnect_ticks, uint32_t tombstone_ticks, bool log_events,
                  uint32_t counts[2]) override {
@@ -1834,6 +2183,30 @@ class CudaBackend : public GsBackend {
     wgraphs_[key] = ge;
     return ge;
   }
+  // The radix sort's scratch, for up to `n` pairs (the pool's capacity): the second key and value buffers,
+  // the per-tile digit counts, every pass's histogram and the plan.  Allocated by the first sort, kept until
+  // the pool is destroyed.
+  bool rs_reserve(size_t n) {
+    if (n <= rs_n_) return true;
+    if (rs_mem_) cudaFree(rs_mem_);
+    rs_mem_ = nullptr;
+    rs_n_ = 0;
+    const size_t nb = (n + GS_RS_TILE - 1) / GS_RS_TILE;
+    const size_t kb = n * 8, vb = (n * 4 + 255) / 256 * 256, hb = (256 * nb * 4 + 255) / 256 * 256;
+    const size_t gb = GS_RS_PASSES * 256 * 4;
+    if (!ok(cudaMalloc(&rs_mem_, kb + vb + hb + gb + sizeof(GsRsCtl)), "radix sort scratch")) {
+      rs_mem_ = nullptr;
+      return false;
+    }
+    uint8_t* q = reinterpret_cast<uint8_t*>(rs_mem_);
+    rs_key_ = reinterpret_cast<uint64_t*>(q);
+    rs_val_ = reinterpret_cast<uint32_t*>(q + kb);
+    rs_hist_ = reinterpret_cast<uint32_t*>(q + kb + vb);
+    rs_ghist_ = reinterpret_cast<uint32_t*>(q + kb + vb + hb);
+    rs_ctl_ = reinterpret_cast<GsRsCtl*>(q + kb + vb + hb + gb);
+    rs_n_ = n;
+    return true;
+  }
   bool ok(cudaError_t e, const char* what) {
     if (e == cudaSuccess) return true;
     snprintf(err_, sizeof(err_), "%s: %s", what, cudaGetErrorString(e));
@@ -1843,6 +2216,13 @@ class CudaBackend : public GsBackend {
   cudaStream_t stream_;
   cudaEvent_t ev0_, ev1_;
   void* scratch_;
+  void* rs_mem_ = nullptr;  // radix sort scratch (rs_reserve)
+  size_t rs_n_ = 0;
+  uint64_t* rs_key_ = nullptr;
+  uint32_t* rs_val_ = nullptr;
+  uint32_t* rs_hist_ = nullptr;
+  uint32_t* rs_ghist_ = nullptr;
+  GsRsCtl* rs_ctl_ = nullptr;
   uint32_t sms_ = 132;
   uint32_t full_grid_ = 528;
   uint32_t win_grid_ = 528;

@@ -24,6 +24,15 @@ FLAG_NO_WINDOWS = 16
 FLAG_PUSH_PULL = 32
 FLAG_COORDINATES = 64
 MEMBER_WATCHED = 1
+MAX_DCS = 64  # datacenters of a latency matrix
+
+
+def _uptr(a: np.ndarray):
+    return a.ctypes.data_as(C.POINTER(C.c_uint32))
+
+
+def _dptr(a: np.ndarray):
+    return a.ctypes.data_as(C.POINTER(C.c_double))
 
 
 class GsimError(RuntimeError):
@@ -174,6 +183,60 @@ class Pool:
         self._ck(self.lib.gsim_coordinate_get(self.h, member, out))
         v = [float(x) for x in out]
         return v[:8], v[8], v[9], v[10]
+
+    # -- network-coordinate queries (read-only; DESIGN.md §3.4 "Queries") ---------------------------
+    def coordinates(self, first: int = 0, count: int | None = None) -> np.ndarray:
+        """Coordinates of members [first, first + count) as rows of (vec[8], error, adjustment, height)."""
+        if count is None:
+            count = self.stats()["n_members"] - first
+        out = np.zeros((max(count, 0), 11), dtype=np.float64)
+        self._ck(self.lib.gsim_coordinates_read(self.h, first, count, _dptr(out)))
+        return out
+
+    def rtt(self, a, b, true_rtt: bool = False):
+        """ComputeDistance between a[k] and b[k] in seconds (`consul rtt`); with true_rtt also the round trip
+        a direct probe samples in the model: (est, true)."""
+        a = np.ascontiguousarray(a, dtype=np.uint32).ravel()
+        b = np.ascontiguousarray(b, dtype=np.uint32).ravel()
+        if a.shape != b.shape:
+            raise ValueError("a and b must have the same length")
+        est = np.zeros(len(a), dtype=np.float64)
+        tru = np.zeros(len(a), dtype=np.float64) if true_rtt else None
+        self._ck(self.lib.gsim_rtt_many(self.h, _uptr(a), _uptr(b), len(a), _dptr(est),
+                                        _dptr(tru) if true_rtt else None))
+        return (est, tru) if true_rtt else est
+
+    def sort_by_distance(self, frm: int, ids=None, k: int | None = None):
+        """sortNodesByDistanceFrom: (ids, distances) of the k nearest of `ids` (None: every member), stable."""
+        if ids is None:
+            n = self.stats()["n_members"]
+            arr = None
+        else:
+            arr = np.ascontiguousarray(ids, dtype=np.uint32).ravel()
+            n = len(arr)
+        k = n if k is None else k
+        out = np.zeros(k, dtype=np.uint32)
+        dist = np.zeros(k, dtype=np.float64)
+        self._ck(self.lib.gsim_sort_by_distance(self.h, frm, _uptr(arr) if arr is not None else None,
+                                                n if arr is not None else 0, k, _uptr(out), _dptr(dist)))
+        return out, dist
+
+    def dcs_by_distance(self, frm: int, servers=None):
+        """Router.GetDatacentersByDistance seen from `frm`: (datacenter indices, median RTTs), nearest first;
+        datacenters without a counted server are left out, as upstream."""
+        order = np.zeros(MAX_DCS, dtype=np.uint32)
+        rtt = np.full(MAX_DCS, np.nan)                 # entries past n_dcs stay NaN
+        arr = None if servers is None else np.ascontiguousarray(servers, dtype=np.uint32).ravel()
+        self._ck(self.lib.gsim_dcs_by_distance(self.h, frm, _uptr(arr) if arr is not None else None,
+                                               0 if arr is None else len(arr), _uptr(order), _dptr(rtt)))
+        keep = np.isfinite(rtt)
+        return order[keep], rtt[keep]
+
+    def coordinate_error(self, n_draws: int, salt: int = 0) -> dict:
+        """Relative error of the embedding against the model's round trips over seeded member pairs."""
+        out = (C.c_double * 6)()
+        self._ck(self.lib.gsim_coordinate_error(self.h, n_draws, salt, out))
+        return dict(zip(("pairs", "mean", "p50", "p90", "p99", "max"), [int(out[0])] + [float(x) for x in out[1:]]))
 
     def latency_set(self, lat):
         """lat: square matrix (n_dcs x n_dcs) of one-way latencies in ticks (>= 1), or None."""

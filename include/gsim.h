@@ -258,6 +258,41 @@ int gsim_member_reconnect_timeout_set(gsim_pool* p, uint32_t id, uint64_t timeou
  * out = {Vec[0..7], Error, Adjustment, Height} in seconds, as coordinate.Coordinate. */
 int gsim_coordinate_get(gsim_pool* p, uint32_t id, double out[11]);
 
+/* Network-coordinate queries at pool scale (DESIGN.md §3.4 "Queries").  Read-only: no pool state, counter,
+ * schedule or digest changes.  Each call is one submission to the device, no per-member round trips.  Pools created
+ * without GSIM_FLAG_COORDINATES return GSIM_ERR_STATE (sharded pools have no coordinates); an id that was
+ * never created is GSIM_ERR_NOT_FOUND.  gsim_sort_by_distance with out_dist copies its two result arrays back
+ * one after the other (one wait each); every other call waits once.  A distance is librtt.ComputeDistance
+ * (internal/gossip/librtt/rtt.go:16-22): Coordinate.DistanceTo(other).Seconds(), through time.Duration.
+ * The first query allocates 12 bytes per member of capacity (plus 12 more on the CUDA backend for its sort). */
+/* (*Serf).GetCoordinate of members [first, first + count): out[11 * x ..] = gsim_coordinate_get(first + x). */
+int gsim_coordinates_read(gsim_pool* p, uint32_t first, uint32_t count, double* out);
+/* `consul rtt` (command/rtt/rtt.go via librtt.ComputeDistance) for n pairs: est_s[k] = the distance between
+ * a[k] and b[k]; true_s[k] (true_s may be NULL) = the round trip a direct probe between them samples in the
+ * model: 0.5 ms + (latency matrix + receive delay, there and back) * tick. */
+int gsim_rtt_many(gsim_pool* p, const uint32_t* a, const uint32_t* b, size_t n, double* est_s, double* true_s);
+/* sortNodesByDistanceFrom (agent/consul/rtt.go:14-52, 190-220), the ?near= order: a stable sort of ids
+ * (NULL: every created member in id order, n ignored) by distance from `from`; the first k results go to
+ * out_ids and out_dist (may be NULL).  GSIM_ERR_INVALID: k > the number of ids, or more ids than capacity. */
+int gsim_sort_by_distance(gsim_pool* p, uint32_t from, const uint32_t* ids, size_t n, size_t k, uint32_t* out_ids,
+                          double* out_dist);
+/* Router.GetDatacentersByDistance (agent/router/router.go:537-615) for one area seen from `from`.  Servers
+ * (NULL: every member, as in a WAN pool) that the view lists Left, or that no longer exist, are skipped; failed
+ * ones count.  Server i is in datacenter (i / 128) % n_dcs; one in from's datacenter counts 0.0.  A
+ * datacenter's RTT is rtts[len / 2] of its sorted RTTs (the upper median).  dc_order / dc_rtt (n_dcs entries
+ * each): datacenters stable-sorted by RTT, ties in index order — the synthetic DC names are ordered by index
+ * where upstream's sort.Strings pass orders names.  A datacenter without a counted server (absent upstream)
+ * comes last, dc_rtt = +inf.  GSIM_ERR_STATE without a latency matrix. */
+int gsim_dcs_by_distance(gsim_pool* p, uint32_t from, const uint32_t* servers, size_t n_servers, uint32_t* dc_order,
+                         double* dc_rtt);
+/* Accuracy of the embedding.  Draw k < n_draws is philox(seed; k, salt, 11) = (x, y, ..): the pair
+ * i = x mod n, j = y mod n, skipped unless i != j and both run.  Over the kept pairs, e = |est - true| / true
+ * (as gsim_rtt_many); out = {pairs kept, mean, p50, p90, p99, max}, order statistic q = the element at
+ * floor(q (m - 1)) of the m ascending errors; the mean adds the errors of each chunk of 256 draws in draw
+ * order, then the chunk sums in chunk order, then divides by m.  NaN statistics when nothing is kept.
+ * GSIM_ERR_INVALID: n_draws == 0 or > capacity. */
+int gsim_coordinate_error(gsim_pool* p, uint32_t n_draws, uint32_t salt, double out[6]);
+
 /* Event logging of one member on/off after creation (that agent's EventCh; see
  * gsim_member_desc.flags / GSIM_MEMBER_WATCHED and gsim_poll_events). */
 int gsim_member_watch(gsim_pool* p, uint32_t id, int on);

@@ -19,6 +19,7 @@
 #include <cstring>
 #include <deque>
 #include <functional>
+#include <limits>
 #include <map>
 #include <memory>
 #include <stdexcept>
@@ -219,6 +220,28 @@ class Serf {
     if (it == p_.by_name_.end()) return false;
     *out = p_.coordinate_of(it->second);
     return true;
+  }
+  // librtt.ComputeDistance(GetCoordinate(), GetCachedCoordinate(name)) — internal/gossip/librtt/rtt.go:16-22,
+  // what `consul rtt` prints: seconds through time.Duration; +inf for a name without a coordinate.
+  double DistanceTo(const std::string& name) {
+    auto it = p_.by_name_.find(name);
+    if (it == p_.by_name_.end()) return std::numeric_limits<double>::infinity();
+    double s = 0.0;
+    p_.check(gsim_rtt_many(p_.h_, &id_, &it->second, 1, &s, nullptr));
+    return s;
+  }
+  // Router.GetDatacentersByDistance() — agent/router/router.go:537-615, for the area of this agent's pool:
+  // datacenter names nearest first by median server RTT (synthetic names "dc<index>", ordered by index on
+  // ties).  Datacenters without a server that counts are left out, as upstream.
+  std::vector<std::string> DatacentersByDistance() {
+    uint32_t order[64];
+    double rtt[64];
+    for (double& r : rtt) r = std::numeric_limits<double>::quiet_NaN();  // entries past n_dcs stay NaN
+    p_.check(gsim_dcs_by_distance(p_.h_, id_, nullptr, 0, order, rtt));
+    std::vector<std::string> out;
+    for (int c = 0; c < 64; ++c)
+      if (std::isfinite(rtt[c])) out.push_back("dc" + std::to_string(order[c]));
+    return out;
   }
   void Leave() { p_.check(gsim_leave(p_.h_, id_)); }
   void Shutdown() { p_.check(gsim_crash(p_.h_, id_)); }  // without Leave(): a crash (server_test.go:725)
