@@ -297,6 +297,11 @@ struct gsim_pool {
   uint32_t* imp_loss = nullptr;
   uint8_t* imp_delay = nullptr;
   uint32_t n_impaired = 0;
+  // ... and the two columns of one-way reachability (gsim_impair_dir_*), allocated by the first setting
+  // whose receive threshold differs from its send threshold or that has a flag: imp_loss is then the send
+  // threshold, imp_recv the receive threshold.  Until then the receive threshold is imp_loss itself.
+  uint32_t* imp_recv = nullptr;
+  uint8_t* imp_flags = nullptr;
   // paused members (gsim_pause_*): the resume-tick column (0 = not paused) and {paused now, resumed Alive,
   // Suspect, Dead}; the first pause allocates the column and pause_cnt_dev, a device copy of the counts that
   // exists only so that snapshots carry them
@@ -1239,12 +1244,21 @@ extern "C" int gsim_join(gsim_pool* p, uint32_t id, const uint32_t* seeds, size_
   const uint32_t cur = p->now & 1u;  // (rows hold key[0] and key[1])
   uint32_t* ri = row(id);
   if (gs_key_truth(ri[cur]) != GS_TRUTH_UP) return fail(p, GSIM_ERR_STATE, "member is not running");
+  // GSIM_IMPAIR_NO_TCP at the joiner or at a seed: the push-pull to that seed cannot connect (only pools
+  // that have the flag column read it)
+  std::vector<uint8_t> no_tcp(ids.size(), 0u);
+  for (size_t x = 0; p->imp_flags && x < ids.size(); ++x) {
+    if (!peek(p, p->imp_flags, ids[x], &no_tcp[x])) return fail(p, GSIM_ERR_CUDA, "peek");
+    no_tcp[x] &= GSIM_IMPAIR_NO_TCP;
+  }
+  auto tcp_blocked = [&](uint32_t m) { return no_tcp[std::find(ids.begin(), ids.end(), m) - ids.begin()] != 0u; };
   int okc = 0;
   for (size_t s = 0; s < n_seeds; ++s) {
     uint32_t sd = seeds[s];
     if (sd >= g.n || sd == id) continue;
     uint32_t* rsd = row(sd);
     if (gs_key_truth(rsd[cur]) != GS_TRUTH_UP) continue;  // unreachable seed: Join skips it
+    if (tcp_blocked(id) || tcp_blocked(sd)) continue;     // ... and so does a seed it cannot connect to
     // push-pull in both directions; eventJoinIgnore applies to the joiner only
     int rc = merge_remote(p, id, rsd, ri, ignore_old != 0);
     if (!rc) rc = merge_remote(p, sd, ri, rsd, false);
@@ -2020,33 +2034,103 @@ static bool impair_alloc(gsim_pool* p) {
   return true;
 }
 
+// The receive-threshold and flag columns, the receive thresholds a copy of the send thresholds (the
+// impairment columns exist already).
+static bool reach_alloc(gsim_pool* p) {
+  if (p->imp_recv) return true;
+  const size_t cap = p->g.cap;
+  uint32_t* recv = nullptr;
+  uint8_t* flags = nullptr;
+  if (!alloc_col(p, &recv, cap) || !alloc_col(p, &flags, cap)) return false;
+  std::vector<uint32_t> loss(cap);
+  if (!dev(p)->d2h(loss.data(), p->imp_loss, cap * 4) || !dev(p)->h2d(recv, loss.data(), cap * 4) ||
+      !dev(p)->fill8(flags, 0, cap))
+    return false;
+  p->imp_recv = recv;
+  p->imp_flags = flags;
+  return true;
+}
+
 // The kernels see the columns only while somebody is impaired: with none, every path (fast paths, long
 // windows, closed form) is exactly the one of a pool that never was.
 static void impair_publish(gsim_pool* p) {
   p->d.imp_loss = p->n_impaired ? p->imp_loss : nullptr;
   p->d.imp_delay = p->n_impaired ? p->imp_delay : nullptr;
+  p->d.imp_recv = p->n_impaired ? (p->imp_recv ? p->imp_recv : p->imp_loss) : nullptr;
+  p->d.imp_flags = p->n_impaired ? p->imp_flags : nullptr;
   mark_dirty(p);
 }
 
+// a member is impaired when any of its four values is non-zero
 static bool impair_recount(gsim_pool* p) {
   p->n_impaired = 0;
   if (p->imp_loss && p->g.n) {
-    std::vector<uint32_t> loss(p->g.n);
-    std::vector<uint8_t> delay(p->g.n);
+    std::vector<uint32_t> loss(p->g.n), recv(p->imp_recv ? p->g.n : 0u);
+    std::vector<uint8_t> delay(p->g.n), flags(p->imp_recv ? p->g.n : 0u);
     if (!dev(p)->d2h(loss.data(), p->imp_loss, loss.size() * 4) || !dev(p)->d2h(delay.data(), p->imp_delay, delay.size()))
       return false;
-    for (uint32_t i = 0; i < p->g.n; ++i) p->n_impaired += (loss[i] | delay[i]) != 0u ? 1u : 0u;
+    if (p->imp_recv && (!dev(p)->d2h(recv.data(), p->imp_recv, recv.size() * 4) ||
+                        !dev(p)->d2h(flags.data(), p->imp_flags, flags.size())))
+      return false;
+    for (uint32_t i = 0; i < p->g.n; ++i)
+      p->n_impaired += (loss[i] | delay[i] | (p->imp_recv ? recv[i] | flags[i] : 0u)) != 0u ? 1u : 0u;
   }
   impair_publish(p);
   return true;
 }
 
-static int impair_check(gsim_pool* p, uint32_t loss_ppm, uint32_t delay_ticks) {
+static int impair_check(gsim_pool* p, uint32_t loss_ppm, uint32_t delay_ticks, uint32_t recv_ppm = 0u,
+                        uint32_t flags = 0u) {
   if (p->sharded) return fail(p, GSIM_ERR_STATE, "member impairment is not supported on sharded pools");
-  if (loss_ppm > 1000000u) return fail(p, GSIM_ERR_INVALID, "loss_ppm must be <= 1000000");
+  if (loss_ppm > 1000000u || recv_ppm > 1000000u) return fail(p, GSIM_ERR_INVALID, "loss_ppm must be <= 1000000");
+  if (flags & ~(uint32_t)GSIM_IMPAIR_NO_TCP) return fail(p, GSIM_ERR_INVALID, "unknown impairment flag");
   // a packet to the member arrives 1 + extra + delay ticks after it was sent: that slot must not wrap the ring
   if ((uint64_t)max_dc_extra(p->g) + delay_ticks + 2u > (uint64_t)p->g.ring_mask + 1u)
     return fail(p, GSIM_ERR_INVALID, "latency plus receive delay must stay below mailbox_depth - 1 extra ticks");
+  return GSIM_OK;
+}
+
+// gsim_impair_many and gsim_impair_dir_many: setting v (thresholds) for the listed members.  A symmetric
+// setting on a pool without the reachability columns touches the two columns it always had.
+static int impair_set_many(gsim_pool* p, const uint32_t* ids, size_t n, const GsImpairVal& v) {
+  for (size_t x = 0; x < n; ++x)
+    if (ids[x] >= p->g.n) return fail(p, GSIM_ERR_NOT_FOUND, "unknown member");
+  const bool now_impaired = (v.send | v.recv | v.delay | v.flags) != 0u;
+  if (!p->imp_loss && !now_impaired) return GSIM_OK;  // clearing on a pool that never was impaired
+  if (!impair_alloc(p)) return fail(p, GSIM_ERR_NOMEM, "impairment columns");
+  if (n && (v.recv != v.send || v.flags != 0u) && !reach_alloc(p))
+    return fail(p, GSIM_ERR_NOMEM, "reachability columns");
+  for (size_t x = 0; x < n; ++x) {
+    uint32_t old_loss, old_recv = 0u;
+    uint8_t old_delay, old_flags = 0u;
+    if (!peek(p, p->imp_loss, ids[x], &old_loss) || !peek(p, p->imp_delay, ids[x], &old_delay))
+      return fail(p, GSIM_ERR_CUDA, "peek");
+    if (p->imp_recv && (!peek(p, p->imp_recv, ids[x], &old_recv) || !peek(p, p->imp_flags, ids[x], &old_flags)))
+      return fail(p, GSIM_ERR_CUDA, "peek");
+    const bool was = (old_loss | old_delay | old_recv | old_flags) != 0u;
+    if (!poke(p, p->imp_loss, ids[x], v.send) || !poke(p, p->imp_delay, ids[x], (uint8_t)v.delay))
+      return fail(p, GSIM_ERR_CUDA, "poke");
+    if (p->imp_recv && (!poke(p, p->imp_recv, ids[x], v.recv) || !poke(p, p->imp_flags, ids[x], (uint8_t)v.flags)))
+      return fail(p, GSIM_ERR_CUDA, "poke");
+    p->n_impaired = p->n_impaired - (was ? 1u : 0u) + (now_impaired ? 1u : 0u);
+  }
+  impair_publish(p);
+  return GSIM_OK;
+}
+
+// gsim_impair_fraction and gsim_impair_dir_fraction: the selection of gs_impair_row, one backend call.
+static int impair_set_fraction(gsim_pool* p, uint32_t member_ppm, uint32_t salt, const GsImpairVal& v,
+                               uint32_t* n_impaired) {
+  if (!impair_alloc(p)) return fail(p, GSIM_ERR_NOMEM, "impairment columns");
+  if ((v.recv != v.send || v.flags != 0u) && !reach_alloc(p)) return fail(p, GSIM_ERR_NOMEM, "reachability columns");
+  if (!upload_globals(p)) return fail(p, GSIM_ERR_CUDA, "upload");
+  uint32_t counts[2] = {0, 0};
+  const GsImpairCols c = {p->imp_loss, p->imp_recv, p->imp_delay, p->imp_flags};
+  if (!dev(p)->impair_dir_fraction(p->d, p->g_dev, p->g, c, ppm_to_thr(member_ppm), salt, v, counts))
+    return fail(p, GSIM_ERR_CUDA, "impair_fraction");
+  p->n_impaired = p->n_impaired - counts[1] + ((v.send | v.recv | v.delay | v.flags) != 0u ? counts[0] : 0u);
+  if (n_impaired) *n_impaired = counts[0];
+  impair_publish(p);
   return GSIM_OK;
 }
 
@@ -2055,24 +2139,17 @@ extern "C" int gsim_impair_many(gsim_pool* p, const uint32_t* ids, size_t n, uin
   std::lock_guard<std::mutex> lk(p->mu);
   int rc = impair_check(p, loss_ppm, delay_ticks);
   if (rc) return rc;
-  for (size_t x = 0; x < n; ++x)
-    if (ids[x] >= p->g.n) return fail(p, GSIM_ERR_NOT_FOUND, "unknown member");
   const uint32_t thr = ppm_to_thr(loss_ppm);
-  const bool now_impaired = thr != 0u || delay_ticks != 0u;
-  if (!p->imp_loss && !now_impaired) return GSIM_OK;  // clearing on a pool that never was impaired
-  if (!impair_alloc(p)) return fail(p, GSIM_ERR_NOMEM, "impairment columns");
-  for (size_t x = 0; x < n; ++x) {
-    uint32_t old_loss;
-    uint8_t old_delay;
-    if (!peek(p, p->imp_loss, ids[x], &old_loss) || !peek(p, p->imp_delay, ids[x], &old_delay))
-      return fail(p, GSIM_ERR_CUDA, "peek");
-    const bool was = old_loss != 0u || old_delay != 0u;
-    if (!poke(p, p->imp_loss, ids[x], thr) || !poke(p, p->imp_delay, ids[x], (uint8_t)delay_ticks))
-      return fail(p, GSIM_ERR_CUDA, "poke");
-    p->n_impaired = p->n_impaired - (was ? 1u : 0u) + (now_impaired ? 1u : 0u);
-  }
-  impair_publish(p);
-  return GSIM_OK;
+  return impair_set_many(p, ids, n, GsImpairVal{thr, thr, delay_ticks, 0u});
+}
+
+extern "C" int gsim_impair_dir_many(gsim_pool* p, const uint32_t* ids, size_t n, uint32_t send_loss_ppm,
+                                    uint32_t recv_loss_ppm, uint32_t delay_ticks, uint32_t flags) {
+  if (!p || (!ids && n)) return GSIM_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(p->mu);
+  int rc = impair_check(p, send_loss_ppm, delay_ticks, recv_loss_ppm, flags);
+  if (rc) return rc;
+  return impair_set_many(p, ids, n, GsImpairVal{ppm_to_thr(send_loss_ppm), ppm_to_thr(recv_loss_ppm), delay_ticks, flags});
 }
 
 extern "C" int gsim_impair_fraction(gsim_pool* p, uint32_t member_ppm, uint32_t salt, uint32_t loss_ppm,
@@ -2081,29 +2158,59 @@ extern "C" int gsim_impair_fraction(gsim_pool* p, uint32_t member_ppm, uint32_t 
   std::lock_guard<std::mutex> lk(p->mu);
   int rc = impair_check(p, loss_ppm, delay_ticks);
   if (rc) return rc;
-  if (!impair_alloc(p)) return fail(p, GSIM_ERR_NOMEM, "impairment columns");
-  if (!upload_globals(p)) return fail(p, GSIM_ERR_CUDA, "upload");
   const uint32_t thr = ppm_to_thr(loss_ppm);
-  uint32_t counts[2] = {0, 0};
-  if (!dev(p)->impair_fraction(p->d, p->g_dev, p->g, p->imp_loss, p->imp_delay, ppm_to_thr(member_ppm), salt, thr,
-                              delay_ticks, counts))
-    return fail(p, GSIM_ERR_CUDA, "impair_fraction");
-  p->n_impaired = p->n_impaired - counts[1] + (thr != 0u || delay_ticks != 0u ? counts[0] : 0u);
-  if (n_impaired) *n_impaired = counts[0];
-  impair_publish(p);
+  return impair_set_fraction(p, member_ppm, salt, GsImpairVal{thr, thr, delay_ticks, 0u}, n_impaired);
+}
+
+extern "C" int gsim_impair_dir_fraction(gsim_pool* p, uint32_t member_ppm, uint32_t salt, uint32_t send_loss_ppm,
+                                        uint32_t recv_loss_ppm, uint32_t delay_ticks, uint32_t flags,
+                                        uint32_t* n_impaired) {
+  if (!p || member_ppm > 1000000u) return GSIM_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(p->mu);
+  int rc = impair_check(p, send_loss_ppm, delay_ticks, recv_loss_ppm, flags);
+  if (rc) return rc;
+  return impair_set_fraction(p, member_ppm, salt,
+                             GsImpairVal{ppm_to_thr(send_loss_ppm), ppm_to_thr(recv_loss_ppm), delay_ticks, flags},
+                             n_impaired);
+}
+
+// the four values of member `id` (thresholds), all zero on a pool that never was impaired
+static int impair_read(gsim_pool* p, uint32_t id, GsImpairVal* v) {
+  if (id >= p->g.n) return fail(p, GSIM_ERR_NOT_FOUND, "unknown member");
+  uint8_t delay = 0, flags = 0;
+  *v = GsImpairVal{0u, 0u, 0u, 0u};
+  if (p->imp_loss && (!peek(p, p->imp_loss, id, &v->send) || !peek(p, p->imp_delay, id, &delay)))
+    return fail(p, GSIM_ERR_CUDA, "peek");
+  v->recv = v->send;
+  if (p->imp_recv && (!peek(p, p->imp_recv, id, &v->recv) || !peek(p, p->imp_flags, id, &flags)))
+    return fail(p, GSIM_ERR_CUDA, "peek");
+  v->delay = delay;
+  v->flags = flags;
   return GSIM_OK;
 }
 
 extern "C" int gsim_impair_get(gsim_pool* p, uint32_t id, uint32_t* loss_ppm, uint32_t* delay_ticks) {
   if (!p) return GSIM_ERR_INVALID;
   std::lock_guard<std::mutex> lk(p->mu);
-  if (id >= p->g.n) return fail(p, GSIM_ERR_NOT_FOUND, "unknown member");
-  uint32_t thr = 0;
-  uint8_t delay = 0;
-  if (p->imp_loss && (!peek(p, p->imp_loss, id, &thr) || !peek(p, p->imp_delay, id, &delay)))
-    return fail(p, GSIM_ERR_CUDA, "peek");
-  if (loss_ppm) *loss_ppm = thr_to_ppm(thr);
-  if (delay_ticks) *delay_ticks = delay;
+  GsImpairVal v;
+  if (int rc = impair_read(p, id, &v)) return rc;
+  if (v.recv != v.send || v.flags != 0u)
+    return fail(p, GSIM_ERR_STATE, "the member's impairment is directional: use gsim_impair_dir_get");
+  if (loss_ppm) *loss_ppm = thr_to_ppm(v.send);
+  if (delay_ticks) *delay_ticks = v.delay;
+  return GSIM_OK;
+}
+
+extern "C" int gsim_impair_dir_get(gsim_pool* p, uint32_t id, uint32_t* send_loss_ppm, uint32_t* recv_loss_ppm,
+                                   uint32_t* delay_ticks, uint32_t* flags) {
+  if (!p) return GSIM_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(p->mu);
+  GsImpairVal v;
+  if (int rc = impair_read(p, id, &v)) return rc;
+  if (send_loss_ppm) *send_loss_ppm = thr_to_ppm(v.send);
+  if (recv_loss_ppm) *recv_loss_ppm = thr_to_ppm(v.recv);
+  if (delay_ticks) *delay_ticks = v.delay;
+  if (flags) *flags = v.flags;
   return GSIM_OK;
 }
 
@@ -3072,7 +3179,7 @@ struct SnapCol {
   uint32_t planes;   // equally sized, each a multiple of 4 bytes
   bool may_fill;     // planes may be stored as a repeated word
 };
-static std::vector<SnapCol> snap_cols(gsim_pool* p, bool with_impairment, bool with_pause) {
+static std::vector<SnapCol> snap_cols(gsim_pool* p, bool with_impairment, bool with_pause, bool with_reach) {
   const GsDev& d = p->d;
   const size_t cap = p->g.cap;
   std::vector<SnapCol> v;
@@ -3099,6 +3206,10 @@ static std::vector<SnapCol> snap_cols(gsim_pool* p, bool with_impairment, bool w
   if (with_impairment) {
     add(p->imp_loss, cap * 4);
     add(p->imp_delay, cap);
+  }
+  if (with_reach) {
+    add(p->imp_recv, cap * 4);
+    add(p->imp_flags, cap);
   }
   if (with_pause) {
     add(p->pause_until, cap * 4);
@@ -3131,6 +3242,7 @@ static uint32_t snap_layout(const gsim_pool* p) {
   if (p->imp_loss) m |= 8u;  // impairment columns (restore allocates them when the pool has none)
   if (p->sharded) m |= 16u;
   if (p->pause_until) m |= 32u;  // the pause column and statistics (restore allocates them when the pool has none)
+  if (p->imp_recv) m |= 64u;     // the reachability columns (with bit 8; restore allocates them when the pool has none)
   return m;
 }
 static uint64_t snap_graph_hash(const gsim_pool* p) {
@@ -3150,7 +3262,8 @@ static uint64_t snap_graph_hash(const gsim_pool* p) {
 static size_t snap_size(gsim_pool* p) {
   size_t s = sizeof(SnapHeader) + p->sched.size() * sizeof(Sched);
   for (uint32_t r = 0; r < GS_MAX_RUMORS; ++r) s += 12 + p->rh[r].name.size() + p->rh[r].payload.size();
-  for (const SnapCol& c : snap_cols(p, p->imp_loss != nullptr, p->pause_until != nullptr)) s += c.bytes + 4u * c.planes;  // upper bound: every plane raw
+  for (const SnapCol& c : snap_cols(p, p->imp_loss != nullptr, p->pause_until != nullptr, p->imp_recv != nullptr))
+    s += c.bytes + 4u * c.planes;  // upper bound: every plane raw
   return s;
 }
 
@@ -3199,7 +3312,7 @@ extern "C" int gsim_snapshot(gsim_pool* p, void* out, size_t cap_bytes, size_t* 
   }
   if (p->pause_cnt_dev && !dev(p)->h2d(p->pause_cnt_dev, p->pause_cnt, sizeof(p->pause_cnt)))
     return fail(p, GSIM_ERR_CUDA, "h2d");
-  for (const SnapCol& c : snap_cols(p, p->imp_loss != nullptr, p->pause_until != nullptr)) {
+  for (const SnapCol& c : snap_cols(p, p->imp_loss != nullptr, p->pause_until != nullptr, p->imp_recv != nullptr)) {
     const size_t pb = c.bytes / c.planes;
     for (uint32_t q = 0; q < c.planes; ++q) {
       uint8_t* raw = w + 4;
@@ -3229,7 +3342,7 @@ extern "C" int gsim_restore(gsim_pool* p, const void* blob, size_t n_bytes) {
   // geometry and peer graph must be this pool's before a single plane is copied.
   if (h.cap != p->g.cap || h.g.cap != p->g.cap || h.g.n > p->cfg.capacity || h.g.n > p->g.cap ||
       h.g.ring_mask != p->g.ring_mask || (h.g.pp_interval != 0u) != (p->g.pp_interval != 0u) ||
-      (h.layout & ~40u) != (snap_layout(p) & ~40u) || h.g.world != p->g.world || h.g.key_stride != p->g.key_stride ||
+      (h.layout & ~104u) != (snap_layout(p) & ~104u) || (h.layout & 72u) == 64u || h.g.world != p->g.world || h.g.key_stride != p->g.key_stride ||
       h.g.rows_per_rank != p->g.rows_per_rank || h.g.phase_group != p->g.phase_group ||
       h.g.graph_n != p->g.graph_n || h.graph_hash != snap_graph_hash(p) || h.n_established > h.g.n)
     return fail(p, GSIM_ERR_INVALID, "snapshot does not match this pool (capacity, column set, sharding or peer graph)");
@@ -3251,9 +3364,11 @@ extern "C" int gsim_restore(gsim_pool* p, const void* blob, size_t n_bytes) {
   }
   const bool blob_impaired = (h.layout & 8u) != 0u;
   if (blob_impaired && !impair_alloc(p)) return fail(p, GSIM_ERR_NOMEM, "impairment columns");
+  const bool blob_reach = (h.layout & 64u) != 0u;
+  if (blob_reach && !reach_alloc(p)) return fail(p, GSIM_ERR_NOMEM, "reachability columns");
   const bool blob_paused = (h.layout & 32u) != 0u;
   if (blob_paused && !pause_alloc(p)) return fail(p, GSIM_ERR_NOMEM, "pause column");
-  for (const SnapCol& c : snap_cols(p, blob_impaired, blob_paused)) {
+  for (const SnapCol& c : snap_cols(p, blob_impaired, blob_paused, blob_reach)) {
     if (c.may_fill) {  // plane by plane: a device fill or a copy
       const size_t pb = c.bytes / c.planes;
       for (uint32_t q = 0; q < c.planes; ++q) {
@@ -3299,6 +3414,13 @@ extern "C" int gsim_restore(gsim_pool* p, const void* blob, size_t n_bytes) {
   // ... and one without the pause column a pool nobody in it is paused
   if (!blob_paused && p->pause_until && !dev(p)->fill32(p->pause_until, 0u, p->g.cap)) return fail(p, GSIM_ERR_CUDA, "fill");
   if (!dev(p)->sync()) return fail(p, GSIM_ERR_CUDA, "sync");  // every plane has left the caller's blob
+  // ... and one without the reachability columns a pool whose settings are all symmetric
+  if (!blob_reach && p->imp_recv) {
+    std::vector<uint32_t> loss(p->g.cap);
+    if (!dev(p)->d2h(loss.data(), p->imp_loss, loss.size() * 4) || !dev(p)->h2d(p->imp_recv, loss.data(), loss.size() * 4) ||
+        !dev(p)->fill8(p->imp_flags, 0, p->g.cap))
+      return fail(p, GSIM_ERR_CUDA, "copy");
+  }
   memset(p->pause_cnt, 0, sizeof(p->pause_cnt));
   if (blob_paused && !dev(p)->d2h(p->pause_cnt, p->pause_cnt_dev, sizeof(p->pause_cnt))) return fail(p, GSIM_ERR_CUDA, "d2h");
   {

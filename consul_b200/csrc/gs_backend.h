@@ -202,26 +202,38 @@ class GsBackend {
   virtual bool xbar_host(const GsXbar&) { return false; }  // arrive, wait for every rank, sync
   virtual bool crash_fraction(const GsDev& d, const GsGlobals* g_dev, const GsGlobals& g,
                               uint32_t thr, uint32_t salt, uint32_t now, uint32_t* n_crashed) = 0;
-  // gs_impair_row over every member, writing the impairment columns (allocated by the caller, who
-  // may not have published them in `d` yet); counts[0] = members selected, counts[1] = how many of
-  // them were impaired before.  Defined here through the copy primitives every backend has, which is
-  // what the host emulation runs; the CUDA backend replaces it with gs_impair_kernel.
-  virtual bool impair_fraction(const GsDev& d, const GsGlobals* /*g_dev*/, const GsGlobals& g, uint32_t* loss_col,
-                               uint8_t* delay_col, uint32_t thr, uint32_t salt, uint32_t loss, uint32_t delay,
-                               uint32_t counts[2]) {
+  // gs_impair_row over every member, writing setting v into the impairment columns c (allocated by the
+  // caller, who may not have published them in `d` yet; c.recv and c.flags may be null); counts[0] =
+  // members selected, counts[1] = how many of them were impaired before.  Defined here through the copy
+  // primitives every backend has, which is what the host emulation runs; the CUDA backend replaces it with
+  // gs_impair_kernel.
+  virtual bool impair_dir_fraction(const GsDev& d, const GsGlobals* /*g_dev*/, const GsGlobals& g,
+                                   const GsImpairCols& c, uint32_t thr, uint32_t salt, const GsImpairVal& v,
+                                   uint32_t counts[2]) {
     counts[0] = counts[1] = 0u;
     if (!g.n) return true;
-    std::vector<uint32_t> key(g.n), lc(g.n);
-    std::vector<uint8_t> dc(g.n);
-    if (!d2h(key.data(), d.key[0], (size_t)g.n * 4) || !d2h(lc.data(), loss_col, (size_t)g.n * 4) ||
-        !d2h(dc.data(), delay_col, g.n))
+    std::vector<uint32_t> key(g.n), lc(g.n), rc(c.recv ? g.n : 0u);
+    std::vector<uint8_t> dc(g.n), fc(c.flags ? g.n : 0u);
+    if (!d2h(key.data(), d.key[0], (size_t)g.n * 4) || !d2h(lc.data(), c.loss, (size_t)g.n * 4) ||
+        !d2h(dc.data(), c.delay, g.n) || (c.recv && !d2h(rc.data(), c.recv, (size_t)g.n * 4)) ||
+        (c.flags && !d2h(fc.data(), c.flags, g.n)))
       return false;
+    const GsImpairCols hc = {lc.data(), c.recv ? rc.data() : nullptr, dc.data(), c.flags ? fc.data() : nullptr};
     for (uint32_t i = 0; i < g.n; ++i) {
-      const uint32_t r = gs_impair_row(key[i], lc.data(), dc.data(), g.seed_lo, g.seed_hi, i, thr, salt, loss, delay);
+      const uint32_t r = gs_impair_row(key[i], hc, g.seed_lo, g.seed_hi, i, thr, salt, v);
       counts[0] += r & 1u;
       counts[1] += (r >> 1) & 1u;
     }
-    return h2d(loss_col, lc.data(), (size_t)g.n * 4) && h2d(delay_col, dc.data(), g.n);
+    return h2d(c.loss, lc.data(), (size_t)g.n * 4) && h2d(c.delay, dc.data(), g.n) &&
+           (!c.recv || h2d(c.recv, rc.data(), (size_t)g.n * 4)) && (!c.flags || h2d(c.flags, fc.data(), g.n));
+  }
+  // The symmetric case (loss, loss, delay, no flags) on the two columns every impaired pool has.
+  virtual bool impair_fraction(const GsDev& d, const GsGlobals* g_dev, const GsGlobals& g, uint32_t* loss_col,
+                               uint8_t* delay_col, uint32_t thr, uint32_t salt, uint32_t loss, uint32_t delay,
+                               uint32_t counts[2]) {
+    const GsImpairCols c = {loss_col, nullptr, delay_col, nullptr};
+    const GsImpairVal v = {loss, loss, delay, 0u};
+    return impair_dir_fraction(d, g_dev, g, c, thr, salt, v, counts);
   }
   // Paused members (gs_aux.h; pause_until is the caller's column).  pause_rows: gs_pause_row(until) over the
   // `n` distinct members ids[] when ids != nullptr, otherwise over every member whose gs_pause_pick(thr, salt)

@@ -286,17 +286,35 @@ GS_HD uint32_t gs_pristine_probes(uint32_t n, uint32_t bits, const GsU4& rk, uin
   return gs_pristine_probes_k(n, bits, rk, self, cursor, (w1 - due + P - 1u) / P, special, n_special);
 }
 
-// gsim_impair_fraction for member i whose key word (either buffer: truth is in both) is key: a member that
-// runs and whose Philox draw (its own purpose word, so the selection is independent of gs_crash_row's for the
-// same salt) is below thr gets the impairment (loss, delay).  Returns bit 0 = selected, bit 1 = it was
-// impaired before.
-GS_HD uint32_t gs_impair_row(uint32_t key, uint32_t* loss_col, uint8_t* delay_col, uint32_t seed_lo, uint32_t seed_hi,
-                             uint32_t i, uint32_t thr, uint32_t salt, uint32_t loss, uint32_t delay) {
+#define GS_IMPAIR_NO_TCP 1u  // GSIM_IMPAIR_NO_TCP: every TCP exchange to or from the member fails
+
+// The impairment columns of a pool (gsim_impair_*, gsim_impair_dir_*): loss = the send threshold, recv and
+// flags null until the first directional setting allocates them (then recv = loss is the symmetric case).
+struct GsImpairCols {
+  uint32_t* loss;
+  uint32_t* recv;
+  uint8_t* delay;
+  uint8_t* flags;
+};
+// The setting written into them: send / receive thresholds, receive delay, GSIM_IMPAIR_* flags.
+struct GsImpairVal {
+  uint32_t send, recv, delay, flags;
+};
+
+// gsim_impair_fraction / gsim_impair_dir_fraction for member i whose key word (either buffer: truth is in
+// both) is key: a member that runs and whose Philox draw (its own purpose word, so the selection is
+// independent of gs_crash_row's for the same salt) is below thr gets the impairment v (recv and flags only
+// where those columns exist).  Returns bit 0 = selected, bit 1 = it was impaired before.
+GS_HD uint32_t gs_impair_row(uint32_t key, const GsImpairCols& c, uint32_t seed_lo, uint32_t seed_hi, uint32_t i,
+                             uint32_t thr, uint32_t salt, const GsImpairVal& v) {
   if ((key & 3u) != GS_TRUTH_UP) return 0u;
   if (gs_philox(seed_lo, seed_hi, i, salt, GS_PUR_IMPAIR, 0u).x >= thr) return 0u;
-  const bool was = loss_col[i] != 0u || delay_col[i] != 0u;
-  loss_col[i] = loss;
-  delay_col[i] = (uint8_t)delay;
+  const bool was = c.loss[i] != 0u || c.delay[i] != 0u || (c.recv != nullptr && c.recv[i] != 0u) ||
+                   (c.flags != nullptr && c.flags[i] != 0u);
+  c.loss[i] = v.send;
+  c.delay[i] = (uint8_t)v.delay;
+  if (c.recv != nullptr) c.recv[i] = v.recv;
+  if (c.flags != nullptr) c.flags[i] = (uint8_t)v.flags;
   return was ? 3u : 1u;
 }
 
@@ -429,7 +447,7 @@ struct GsDev {
   // degraded members (gsim_impair_*): per-member UDP loss threshold and receive delay in ticks.  Both
   // null unless at least one member is impaired right now, which is also what turns the probe fast
   // paths off (the host keeps the columns and the count; a pool that was never impaired has neither).
-  const uint32_t* imp_loss;  // [cap] packet to or from the member lost iff a Philox word < imp_loss
+  const uint32_t* imp_loss;  // [cap] packet from the member lost iff Philox word y < imp_loss (send threshold)
   const uint8_t* imp_delay;  // [cap] extra ticks before the member handles what it receives
   // pool-wide device words
   unsigned long long* stats;  // [GSIM_STAT_COUNT]
@@ -447,6 +465,12 @@ struct GsDev {
   // quiet-window scheduling (DESIGN.md §4.2): qstate[r] = rank r's copy of the GS_Q_* words; this
   // rank reads qstate[rank], writers update every rank's copy (like key_rep)
   uint32_t* qstate[GS_MAX_WORLD_];
+  // one-way reachability (gsim_impair_dir_*), set exactly when imp_loss is: packet to the member lost iff
+  // Philox word z < imp_recv (imp_recv == imp_loss until some member's receive threshold differs from its
+  // send threshold or has a flag), and GSIM_IMPAIR_* flags per member (null until the first directional
+  // setting).  Last in the struct, so every other field keeps its offset.
+  const uint32_t* imp_recv;
+  const uint8_t* imp_flags;
 };
 
 // Pool-wide scheduling words (one copy per rank).  A pool is QUIET when every mailbox slot is empty

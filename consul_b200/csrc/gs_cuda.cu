@@ -992,12 +992,14 @@ __global__ void __launch_bounds__(GS_BLOCK)
   if ((threadIdx.x & 31u) == 0u && b) atomicAdd(n_crashed, (uint32_t)__popc(b));
 }
 
+// gsim_impair_fraction / gsim_impair_dir_fraction: gs_impair_row for member i, counts[0] += selected,
+// counts[1] += selected members that were impaired before.
 __global__ void __launch_bounds__(GS_BLOCK)
-    gs_impair_kernel(GsDev d, const GsGlobals* __restrict__ gp, uint32_t* loss_col, uint8_t* delay_col, uint32_t thr,
-                     uint32_t salt, uint32_t loss, uint32_t delay, uint32_t* counts) {
+    gs_impair_kernel(GsDev d, const GsGlobals* __restrict__ gp, GsImpairCols c, uint32_t thr, uint32_t salt,
+                     GsImpairVal v, uint32_t* counts) {
   const uint32_t i = blockIdx.x * GS_BLOCK + threadIdx.x;
   uint32_t r = 0u;
-  if (i < gp->n) r = gs_impair_row(d.key[0][i], loss_col, delay_col, gp->seed_lo, gp->seed_hi, i, thr, salt, loss, delay);
+  if (i < gp->n) r = gs_impair_row(d.key[0][i], c, gp->seed_lo, gp->seed_hi, i, thr, salt, v);
   const unsigned sel = __ballot_sync(0xFFFFFFFFu, r & 1u), was = __ballot_sync(0xFFFFFFFFu, r & 2u);
   if ((threadIdx.x & 31u) == 0u && sel) {
     atomicAdd(&counts[0], (uint32_t)__popc(sel));
@@ -1798,15 +1800,13 @@ class CudaBackend : public GsBackend {
     }
     return ok(cudaGetLastError(), "crash launch") && d2h(n_crashed, cnt, 4);
   }
-  bool impair_fraction(const GsDev& d, const GsGlobals* g_dev, const GsGlobals& g, uint32_t* loss_col,
-                       uint8_t* delay_col, uint32_t thr, uint32_t salt, uint32_t loss, uint32_t delay,
-                       uint32_t counts[2]) override {
+  bool impair_dir_fraction(const GsDev& d, const GsGlobals* g_dev, const GsGlobals& g, const GsImpairCols& c,
+                           uint32_t thr, uint32_t salt, const GsImpairVal& v, uint32_t counts[2]) override {
     cudaSetDevice(dev_);
     uint32_t* cnt = reinterpret_cast<uint32_t*>(scratch_);
     if (!ok(cudaMemsetAsync(cnt, 0, 8, stream_), "memset")) return false;
     if (g.n) {
-      gs_impair_kernel<<<(g.n + GS_BLOCK - 1) / GS_BLOCK, GS_BLOCK, 0, stream_>>>(d, g_dev, loss_col, delay_col, thr,
-                                                                                  salt, loss, delay, cnt);
+      gs_impair_kernel<<<(g.n + GS_BLOCK - 1) / GS_BLOCK, GS_BLOCK, 0, stream_>>>(d, g_dev, c, thr, salt, v, cnt);
       ++launches_;
     }
     return ok(cudaGetLastError(), "impair launch") && d2h(counts, cnt, 8);

@@ -206,31 +206,44 @@ GS_DEV uint32_t gs_extra(const G& g, const uint8_t* delay, uint32_t src, uint32_
   return e;
 }
 
+// The per-member loss thresholds of a pool with impaired members: the sender's send threshold and
+// the receiver's receive threshold (GsDev::imp_loss / imp_recv, the same column while every setting
+// is symmetric); send == null while nobody is impaired.
+struct GsLossCols {
+  const uint32_t* send;
+  const uint32_t* recv;
+};
+
 // The loss rule of one simulated UDP packet from src to dst, on Philox block r of its counter: the
-// pool-wide draw (r.x), then the sender's and the receiver's own loss (r.y, r.z; `loss` =
-// GsDev::imp_loss, null while nobody is impaired).
-GS_DEV bool gs_loss_rule(const GsGlobals& g, const uint32_t* loss, const GsU4& r, uint32_t src, uint32_t dst) {
-  return r.x < g.loss_thr || (loss != nullptr && (r.y < loss[src] || r.z < loss[dst]));
+// pool-wide draw (r.x), then the sender's send threshold (r.y) and the receiver's receive threshold (r.z).
+GS_DEV bool gs_loss_rule(const GsGlobals& g, const GsLossCols& loss, const GsU4& r, uint32_t src, uint32_t dst) {
+  return r.x < g.loss_thr || (loss.send != nullptr && (r.y < loss.send[src] || r.z < loss.recv[dst]));
 }
 
 // Same draw as gs_lost without touching the counters: re-evaluates, at the ProbeTimeout stage,
 // whether the direct ping/ack of the probe started at t0 were lost (late acks, latency pools).
-GS_DEV bool gs_lost_quiet(const GsGlobals& g, const uint32_t* loss, uint32_t src, uint32_t dst, uint32_t t,
+GS_DEV bool gs_lost_quiet(const GsGlobals& g, const GsLossCols& loss, uint32_t src, uint32_t dst, uint32_t t,
                           uint32_t kind, uint32_t idx) {
-  if (g.loss_thr == 0u && loss == nullptr) return false;
+  if (g.loss_thr == 0u && loss.send == nullptr) return false;
   GsU4 r = gs_philox(g.seed_lo, g.seed_hi, src, dst, t, GS_PUR_LOSS | (kind << 8) | (idx << 16));
   return gs_loss_rule(g, loss, r, src, dst);
 }
 
 // One simulated UDP packet is lost iff its Philox draw says so (gs_loss_rule); counted once.
 template <class Sink>
-GS_DEV bool gs_lost(const GsGlobals& g, const uint32_t* loss, Sink& sink, uint32_t src, uint32_t dst, uint32_t t,
+GS_DEV bool gs_lost(const GsGlobals& g, const GsLossCols& loss, Sink& sink, uint32_t src, uint32_t dst, uint32_t t,
                     uint32_t kind, uint32_t idx) {
-  if (g.loss_thr == 0u && loss == nullptr) return false;
+  if (g.loss_thr == 0u && loss.send == nullptr) return false;
   GsU4 r = gs_philox(g.seed_lo, g.seed_hi, src, dst, t, GS_PUR_LOSS | (kind << 8) | (idx << 16));
   bool lost = gs_loss_rule(g, loss, r, src, dst);
   if (lost) sink.stat(GS_ST_PACKETS_LOST, 1);
   return lost;
+}
+
+// Does a TCP exchange between members i and j fail (GSIM_IMPAIR_NO_TCP at either end)?  `flags` =
+// GsDev::imp_flags, null unless some member has a directional setting.
+GS_DEV bool gs_no_tcp(const uint8_t* flags, uint32_t i, uint32_t j) {
+  return flags != nullptr && ((flags[i] | flags[j]) & GS_IMPAIR_NO_TCP) != 0u;
 }
 
 // Does member i know member c exists?  Established members are known to everyone; a
@@ -458,14 +471,15 @@ GS_DEV bool gs_mail_is_stale(const GsGlobals& g, uint32_t w, uint32_t heard, boo
 // The tick of member i, called only for rows that have mail (inb = inbox[t&1][i] != 0,
 // which includes the self-posted wake bit) or a probe action due (due[i] == t).  Stale mail
 // (gs_mail_is_stale) only clears the word; the tick kernel's scan retires it without calling here.
-// IMPAIRED: the pool has degraded members (GsDev::imp_loss / imp_delay are set).  The other
-// instantiation folds every impairment term away, so a pool without any runs the code it would
-// run without the feature.
+// IMPAIRED: the pool has degraded members (GsDev::imp_loss / imp_recv / imp_delay are set, imp_flags
+// when some member has a directional setting).  The other instantiation folds every impairment term
+// away, so a pool without any runs the code it would run without the feature.
 template <bool IMPAIRED, class Sink>
 GS_DEV void gs_row_step_body(const GsDev& d, const GsGlobals& g, uint32_t i, uint32_t t, uint32_t gslot,
                              uint32_t inb, Sink& sink) {
-  const uint32_t* const imp_loss = IMPAIRED ? d.imp_loss : nullptr;
+  const GsLossCols imp_loss = {IMPAIRED ? d.imp_loss : nullptr, IMPAIRED ? d.imp_recv : nullptr};
   const uint8_t* const imp_delay = IMPAIRED ? d.imp_delay : nullptr;
+  const uint8_t* const imp_flags = IMPAIRED ? d.imp_flags : nullptr;
   const uint32_t cur = t & 1u, nxt = cur ^ 1u;                            // key / acc buffers
   const uint32_t icur = t & g.ring_mask, inxt = (t + 1u) & g.ring_mask;  // mailbox ring slots
   const uint32_t k0 = d.key[cur][i];
@@ -687,7 +701,8 @@ GS_DEV void gs_row_step_body(const GsDev& d, const GsGlobals& g, uint32_t i, uin
       }
       const uint32_t t0 = t - g.T;
       const uint32_t rtt_ij = gs_extra(g, imp_delay, i, j) + gs_extra(g, imp_delay, j, i);
-      if (!g.disable_tcp && j_up && rtt_ij <= budget) success = true;  // TCP fallback ping is reliable
+      // TCP fallback ping: reliable, unless either end has TCP blocked (GSIM_IMPAIR_NO_TCP)
+      if (!g.disable_tcp && j_up && rtt_ij <= budget && !gs_no_tcp(imp_flags, i, j)) success = true;
       // a direct ack that was merely slower than ProbeTimeout still counts until the deadline
       if ((g.n_dcs != 0u || imp_delay != nullptr) && j_up && rtt_ij > g.T && rtt_ij <= budget + g.T &&
           !gs_lost_quiet(g, imp_loss, i, j, t0, GS_LK_PING, 0) && !gs_lost_quiet(g, imp_loss, j, i, t0, GS_LK_ACK, 0))
@@ -874,17 +889,21 @@ GS_DEV void gs_row_step_body(const GsDev& d, const GsGlobals& g, uint32_t i, uin
       uint32_t partner[1];
       if (gs_krandom(d, g, i, t, GS_PUR_PUSHPULL, 1u, 1u, GS_EMPTY32, m, partner) != 0u) {
         const uint32_t j = partner[0];
-        uint32_t* req = d.ppreq + (size_t)nxt * GS_PPK * cap;
-        uint32_t v = i;
-        for (uint32_t s = 0; s < GS_PPK; ++s) {
-          const uint32_t old = GS_ATOMIC_MIN32(&req[(size_t)s * cap + j], v);
-          if (old == v || old == GS_EMPTY32) break;
-          if (old > v) v = old;  // displaced a larger id: carry it to the next slot
+        // an end that cannot use TCP (GSIM_IMPAIR_NO_TCP): the exchange is started and counted, but
+        // nothing is pushed and nothing comes back
+        if (!gs_no_tcp(imp_flags, i, j)) {
+          uint32_t* req = d.ppreq + (size_t)nxt * GS_PPK * cap;
+          uint32_t v = i;
+          for (uint32_t s = 0; s < GS_PPK; ++s) {
+            const uint32_t old = GS_ATOMIC_MIN32(&req[(size_t)s * cap + j], v);
+            if (old == v || old == GS_EMPTY32) break;
+            if (old > v) v = old;  // displaced a larger id: carry it to the next slot
+          }
+          uint32_t* clk = d.pp_clk + (size_t)nxt * 2u * cap;
+          GS_ATOMIC_MAX32(&clk[j], d.ltime_member[i]);
+          GS_ATOMIC_MAX32(&clk[cap + j], d.ltime_event[i]);
+          gs_post(d, g, sink, inxt, j, (d.heard[i] & g.active_mask) | GS_ACC_BIT);
         }
-        uint32_t* clk = d.pp_clk + (size_t)nxt * 2u * cap;
-        GS_ATOMIC_MAX32(&clk[j], d.ltime_member[i]);
-        GS_ATOMIC_MAX32(&clk[cap + j], d.ltime_event[i]);
-        gs_post(d, g, sink, inxt, j, (d.heard[i] & g.active_mask) | GS_ACC_BIT);
         sink.stat(GS_ST_PUSH_PULLS, 1);
       }
     }

@@ -13,6 +13,8 @@ from . import _lib
 from ._lib import (COLUMNS, GSIM_MAX_RUMORS, GSIM_MAX_SUSPICION_SLOTS, STAT_NAMES, GsimConfig,
                    GsimEvent, GsimMember, GsimMemberDesc, GsimRumorInfo, GsimStats)
 
+IMPAIR_NO_TCP = 1  # GSIM_IMPAIR_NO_TCP
+
 PRED_RUMOR_CONVERGED = 1
 PRED_ALL_RUMORS_CONVERGED = 2
 PRED_CRASHED_ALL_DEAD = 3
@@ -264,6 +266,29 @@ class Pool:
         loss, delay = C.c_uint32(), C.c_uint32()
         self._ck(self.lib.gsim_impair_get(self.h, member, C.byref(loss), C.byref(delay)))
         return loss.value, delay.value
+
+    def impair_dir(self, ids, send_loss_ppm: int, recv_loss_ppm: int, delay_ticks: int = 0, no_tcp: bool = False):
+        """One-way reachability for the listed members: UDP loss of what each sends and of what it
+        receives (ppm), a receive delay (ticks) and, with no_tcp, no TCP to or from it (no fallback
+        ping, no push-pull, no join through it).  (0, 0, 0, False) clears it."""
+        arr = (C.c_uint32 * max(1, len(ids)))(*ids)
+        self._ck(self.lib.gsim_impair_dir_many(self.h, arr, len(ids), send_loss_ppm, recv_loss_ppm, delay_ticks,
+                                               IMPAIR_NO_TCP if no_tcp else 0))
+
+    def impair_dir_fraction(self, member_ppm: int, salt: int, send_loss_ppm: int, recv_loss_ppm: int,
+                            delay_ticks: int = 0, no_tcp: bool = False) -> int:
+        """impair_dir on the members impair_fraction selects for the same salt; returns how many."""
+        out = C.c_uint32()
+        self._ck(self.lib.gsim_impair_dir_fraction(self.h, member_ppm, salt, send_loss_ppm, recv_loss_ppm,
+                                                   delay_ticks, IMPAIR_NO_TCP if no_tcp else 0, C.byref(out)))
+        return out.value
+
+    def impairment_dir(self, member: int):
+        """(send_loss_ppm, recv_loss_ppm, delay_ticks, no_tcp) of one member, as set."""
+        send, recv, delay, flags = C.c_uint32(), C.c_uint32(), C.c_uint32(), C.c_uint32()
+        self._ck(self.lib.gsim_impair_dir_get(self.h, member, C.byref(send), C.byref(recv), C.byref(delay),
+                                              C.byref(flags)))
+        return send.value, recv.value, delay.value, bool(flags.value & IMPAIR_NO_TCP)
 
     def pause(self, ids, ticks: int) -> int:
         """Stop the listed members (running, not leaving) for `ticks` ticks; returns how many were paused."""

@@ -336,8 +336,37 @@ int gsim_impair_many(gsim_pool* p, const uint32_t* ids, size_t n, uint32_t loss_
  * independent of gsim_crash_fraction's for the same salt); *n_impaired = members selected. */
 int gsim_impair_fraction(gsim_pool* p, uint32_t member_ppm, uint32_t salt, uint32_t loss_ppm, uint32_t delay_ticks,
                          uint32_t* n_impaired);
-/* The impairment of member `id` exactly as it was set. */
+/* The impairment of member `id` exactly as it was set.  GSIM_ERR_STATE when the member's setting is
+ * directional (send and receive loss differ, or a flag is set): use gsim_impair_dir_get. */
 int gsim_impair_get(gsim_pool* p, uint32_t id, uint32_t* loss_ppm, uint32_t* delay_ticks);
+
+/* One-way reachability (DESIGN.md §3.5 "One-way reachability"): the impairment of member m split by
+ * direction, (send_loss_ppm[m], recv_loss_ppm[m], delay[m], flags[m]).  gsim_impair_many and
+ * gsim_impair_fraction set the symmetric case (loss, loss, delay, 0) of the same rules.
+ *  - UDP: a packet src -> dst on Philox block r is lost iff r.x < thr(packet_loss_ppm), or
+ *    r.y < thr(send_loss_ppm[src]), or r.z < thr(recv_loss_ppm[dst]), on every leg the loss rule above
+ *    covers.  A symmetric setting therefore gives exactly the draws of gsim_impair_many.
+ *  - GSIM_IMPAIR_NO_TCP: every TCP exchange to or from the member fails.  The TCP fallback ping of a probe
+ *    between i and j fails when either has it; a push-pull that i opens with partner j exchanges nothing
+ *    (the partner is drawn and GSIM_STAT_PUSH_PULLS counts the exchange as before); gsim_join skips a seed
+ *    when the seed or the joiner has it, like an unreachable seed.
+ *  - Accusations, wake bits and host operations stay lossless and the receive delay stays receive-only, so
+ *    a member that runs is still never declared Failed (see gsim_impair_many).
+ *  - A member counts as impaired when any of its four values is non-zero: GSIM_IMPAIR_NO_TCP alone turns
+ *    the probe fast paths and long quiet windows off pool-wide, as loss does.
+ *  - Columns: the first setting with send != recv or a flag allocates 4 + 1 more bytes per member;
+ *    gsim_snapshot then carries them.  Validation, GSIM_ERR_NOT_FOUND and the sharded refusal as for
+ *    gsim_impair_many; GSIM_ERR_INVALID for a flag bit other than GSIM_IMPAIR_NO_TCP.
+ *  - Measured (one H100 80GB HBM3, 700 W, DESIGN.md §6): 1 Mi LAN members with 1 % inbound-blocked give no
+ *    suspicion with the TCP fallback, and 1.84 M false suspicions over 3 000 ticks without it. */
+#define GSIM_IMPAIR_NO_TCP 1u
+int gsim_impair_dir_many(gsim_pool* p, const uint32_t* ids, size_t n, uint32_t send_loss_ppm, uint32_t recv_loss_ppm,
+                         uint32_t delay_ticks, uint32_t flags);
+/* The selection of gsim_impair_fraction (the same salt picks the same members). */
+int gsim_impair_dir_fraction(gsim_pool* p, uint32_t member_ppm, uint32_t salt, uint32_t send_loss_ppm,
+                             uint32_t recv_loss_ppm, uint32_t delay_ticks, uint32_t flags, uint32_t* n_impaired);
+int gsim_impair_dir_get(gsim_pool* p, uint32_t id, uint32_t* send_loss_ppm, uint32_t* recv_loss_ppm,
+                        uint32_t* delay_ticks, uint32_t* flags);
 
 /* Paused members (simulator-only fault injection: a GC pause, a VM steal, a SIGSTOP; DESIGN.md §3.6):
  * a member paused at tick t0 for d ticks is a stopped process during ticks t0 .. t0+d-1 and carries on
