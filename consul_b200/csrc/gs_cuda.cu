@@ -224,10 +224,14 @@ __global__ void __launch_bounds__(GS_BLOCK, GS_MIN_BLOCKS)
   __shared__ __align__(128) uint32_t s_due[GS_WARPS][GS_ROUND][GS_TILE];  // ... and `due` words (gated tiles only)
   __shared__ __align__(8) uint64_t s_bar[GS_WARPS];                       // one transaction barrier per warp
   __shared__ uint32_t s_q[2];
-  // groups of 32 members that need the generic step, queued by the scanning warps and taken by
-  // whichever warp of the CTA is free (two counters each: rounds alternate, see below)
-  __shared__ uint32_t s_work[GS_WARPS * GS_ROUND * 4];
+  // members that need the generic step, queued one entry each by the scanning warps and taken 32 at a time
+  // by whichever warp of the CTA is free (two counters each: rounds alternate, see below).  An entry is
+  // (scanning warp << 9) | (tile in its round << 7) | member in tile; s_rtile[w] is warp w's first tile
+  // of the round.
+  __shared__ uint16_t s_work[GS_WARPS * GS_ROUND * GS_TILE];
+  __shared__ uint32_t s_rtile[GS_WARPS];
   __shared__ uint32_t s_wn[2], s_wtake[2];
+  static_assert(GS_WARPS <= 8 && GS_ROUND <= 4 && GS_TILE == 128, "s_work entries are 3 + 2 + 7 bits");
   const uint32_t tid = threadIdx.x;
   for (uint32_t x = tid; x < GS_NSTAT * 32u; x += GS_BLOCK) s_stat[x] = 0u;
   for (uint32_t x = tid; x < 32u * 32u; x += GS_BLOCK) s_heard[x] = 0u;
@@ -275,11 +279,13 @@ __global__ void __launch_bounds__(GS_BLOCK, GS_MIN_BLOCKS)
   DevSinkT<COORDS> sink{s_stat, s_heard, s_q};
 
   // Rounds.  A warp scans up to GS_ROUND of its tiles and runs the staged probe fast path inline;
-  // every group that needs the generic step goes into the CTA's queue instead.  Then the whole CTA
-  // drains the queue, one group per warp at a time: a warp whose tiles were idle helps the warp whose
-  // tiles all gossip (ticker phases come in runs of ProbeInterval tiles, so consecutive tiles are
-  // busy together and a static split leaves half the warps waiting at the closing barrier).  Results
-  // do not depend on who steps a group: everything a member sends is a commutative atomic.
+  // every member that needs the generic step goes into the CTA's queue instead.  Then the whole CTA
+  // drains the queue, 32 members per warp at a time: a warp whose tiles were idle helps the warp whose
+  // tiles all gossip (gossip phases come in runs of ProbeInterval tiles, so consecutive tiles are
+  // busy together and a static split leaves half the warps waiting at the closing barrier), and in the
+  // rise and the tail of a join cascade, when a few active members are spread over every 32-member
+  // group, a warp-step still steps 32 of them.  Results do not depend on who steps a member:
+  // everything a member sends is a commutative atomic and counters are summed per lane.
   const uint32_t max_run = (n_tiles + n_warps - 1u) / n_warps, n_rounds = (max_run + GS_ROUND - 1u) / GS_ROUND;
   bool did_work = false;  // this thread touched global state (needs the closing fence when sharded)
   const bool sys_scan = g.world > 1u && (g.flags & 4u);  // GSIM_FLAG_SHARD_SYNC_SCAN (debug): system-scope loads, no bulk copy
@@ -416,30 +422,47 @@ __global__ void __launch_bounds__(GS_BLOCK, GS_MIN_BLOCKS)
           if (n_ack) atomicAdd(&s_stat[GS_ST_ACKS * 32], n_ack);
         }
       }
+      // queue the members left (mail, a probe action the fast path declined, the push-pull ticker): one
+      // shared atomic reserves the tile's entries, each active lane writes its own at its prefix position
+      uint32_t bal[4], n_act = 0;
 #pragma unroll
       for (int u = 0; u < 4; ++u) {
-        if (__any_sync(0xFFFFFFFFu, act[u]) && lane == 0u) s_work[atomicAdd(&s_wn[par], 1u)] = tile * 4u + (uint32_t)u;
+        bal[u] = __ballot_sync(0xFFFFFFFFu, act[u]);
+        n_act += __popc(bal[u]);
+      }
+      if (n_act) {
+        uint32_t pos = 0;
+        if (lane == 0u) pos = atomicAdd(&s_wn[par], n_act);
+        pos = __shfl_sync(0xFFFFFFFFu, pos, 0);
+        const uint32_t below = (1u << lane) - 1u, key = (wib << 9) | (st << 7) | lane;
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+          if (act[u]) s_work[pos + __popc(bal[u] & below)] = (uint16_t)(key | ((uint32_t)u << 5));
+          pos += __popc(bal[u]);
+        }
       }
     }
   }
+  if (lane == 0u) s_rtile[wib] = r_begin;
   __syncwarp();                              // this warp is done with its round buffers:
   if (round + 1u < n_rounds) bring(round + 1u);  // the next round's copy flies while the CTA drains its queue
   __syncthreads();  // the queue of this round is complete
   if (tid == 0u) s_wn[par ^ 1u] = s_wtake[par ^ 1u] = 0u;  // the next round's counters (nobody uses them now)
   const uint32_t n_work = s_wn[par];
+  // Drain: 32 queued members per warp-step, whichever tiles and scanning warps they came from.  Every lane
+  // with an entry steps its member.  The mailbox word is re-read: the round buffer may already hold the next
+  // round's copy, and stale mail was cleared in global memory before the barrier above.
   for (;;) {
     uint32_t idx = 0;
-    if (lane == 0u) idx = atomicAdd(&s_wtake[par], 1u);
+    if (lane == 0u) idx = atomicAdd(&s_wtake[par], 32u);
     idx = __shfl_sync(0xFFFFFFFFu, idx, 0);
     if (idx >= n_work) break;
     did_work = true;
-    const uint32_t i = s_work[idx] * 32u + lane;
-    // which members of the group: mail, a probe action due (members the fast path finished have moved
-    // their `due` on), or the push-pull ticker
-    const uint32_t w = __ldcg(inbox_cur + i);
-    const bool a = w != 0u || __ldcg(d.due + i) == t ||
-                   (g.pp_interval != 0u && gs_pp_due(g.pp_interval, g.rot_pp, i / g.phase_group, t));
-    if (a) gs_row_step_call<COORDS>(&d, gp, i, t, w, s_stat, s_heard, s_q);
+    if (idx + lane < n_work) {
+      const uint32_t e = s_work[idx + lane];
+      const uint32_t i = (s_rtile[e >> 9] + ((e >> 7) & 3u)) * GS_TILE + (e & 127u);
+      gs_row_step_call<COORDS>(&d, gp, i, t, __ldcg(inbox_cur + i), s_stat, s_heard, s_q);
+    }
   }
   __syncthreads();  // the queue is drained (and its counters may be reused two rounds from now)
   }  // rounds
