@@ -44,11 +44,16 @@ __device__ __forceinline__ uint64_t gs_atomic_min_sys(uint64_t* p, uint64_t v) {
 __device__ __forceinline__ void gs_red_or_sys(uint32_t* p, uint32_t v) {
   asm volatile("red.global.sys.or.b32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
+// Single-GPU posts: the same reduction at device scope (atomicOr on a generic pointer whose result is
+// unused is still a generic fetching ATOM).
+__device__ __forceinline__ void gs_red_or_gpu(uint32_t* p, uint32_t v) {
+  asm volatile("red.global.gpu.or.b32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
 // (`g` is the GsGlobals in scope at every use: single-GPU pools keep the cheap device-scope forms)
 #define GS_ATOMIC_OR32(p, v) (g.world > 1u ? gs_atomic_or_sys((p), (v)) : atomicOr((p), (v)))
 #define GS_POST_OR32(p, v)                                                         \
   do {                                                                             \
-    if (g.world <= 1u) (void)atomicOr((p), (v));                                   \
+    if (g.world <= 1u) gs_red_or_gpu((p), (v));                                    \
     else if (g.flags & 128u) (void)gs_atomic_or_sys((p), (v));                     \
     else gs_red_or_sys((p), (v));                                                  \
   } while (0)
@@ -482,7 +487,12 @@ GS_DEV void gs_row_step_body(const GsDev& d, const GsGlobals& g, uint32_t i, uin
   const uint8_t* const imp_flags = IMPAIRED ? d.imp_flags : nullptr;
   const uint32_t cur = t & 1u, nxt = cur ^ 1u;                            // key / acc buffers
   const uint32_t icur = t & g.ring_mask, inxt = (t + 1u) & g.ring_mask;  // mailbox ring slots
-  const uint32_t k0 = d.key[cur][i];
+  // The row's own words are loaded together, before anything is stored and before any test looks at one
+  // of them (i < cap for every row stepped, so the loads are safe whatever the tests decide): one memory
+  // latency, not three.  `heard` only when the arrival carries tracked rumor bits.
+  const uint32_t rbits = inb & ~(GS_ACC_BIT | GS_WAKE_BIT) & g.active_mask;
+  const uint32_t k0 = d.key[cur][i], m0 = d.meta[i], due0 = d.due[i], queued0 = d.queued[i];
+  const uint32_t heard0 = rbits != 0u ? d.heard[i] : 0u;
   const uint32_t truth = gs_key_truth(k0);
   if (inb != 0u) sink.activity();
   if (truth == GS_TRUTH_NONE) {
@@ -491,14 +501,9 @@ GS_DEV void gs_row_step_body(const GsDev& d, const GsGlobals& g, uint32_t i, uin
     if (inb != 0u) d.inbox[icur][i] = 0u;
     return;
   }
-  const uint32_t m0 = d.meta[i];
-  const uint32_t due0 = d.due[i];
   const bool up = truth == GS_TRUTH_UP;
   const bool gossip_slot = up && gslot == gs_meta_gphase(m0);  // gslot = t % GI
-  uint32_t queued = up ? d.queued[i] : 0u;
-  // the tracked rumor bits of this arrival tick and, when there are any, what the member has heard
-  const uint32_t rbits = inb & ~(GS_ACC_BIT | GS_WAKE_BIT) & g.active_mask;
-  const uint32_t heard0 = rbits != 0u ? d.heard[i] : 0u;
+  uint32_t queued = up ? queued0 : 0u;
   if (inb != 0u) d.inbox[icur][i] = 0u;
   // periodic push-pull (opt-in): does this member's push-pull ticker fire now?
   const bool pp_now = up && g.pp_interval != 0u && gs_pp_due(g.pp_interval, g.rot_pp, i / g.phase_group, t);
@@ -800,29 +805,39 @@ GS_DEV void gs_row_step_body(const GsDev& d, const GsGlobals& g, uint32_t i, uin
     if (gossip_slot && queued != 0u) {
       uint32_t peers[8];
       uint32_t kk = g.gossip_nodes > 8u ? 8u : g.gossip_nodes;
-      uint32_t np = gs_krandom(d, g, i, t, GS_PUR_GOSSIP, kk, 0u, GS_EMPTY32, m, peers);
-      const uint32_t q0 = queued;
-      if (g.active_bytes <= g.udp_avail && np != 0u) {
-        // Every packet carries the whole queue (the byte budget cannot bind).  Broadcast r then rides
-        // in packets 0 .. sends_r - 1 with sends_r = min(np, max(1, limit - transmits_r)): one read
-        // and one write of its counter instead of one per packet, same counters and same packets as
-        // the general loop below.
-        uint32_t sends[GS_MAX_RUMORS > 8 ? 8 : GS_MAX_RUMORS];
-        uint32_t n_pkts = 0, n_q = 0, pm = queued;
-        bool few = true;
-        while (pm) {
+      // Every packet carries the whole queue when the byte budget cannot bind: then the transmit counters
+      // of the first eight queued broadcasts (one byte each) are all that this section reads of the row,
+      // and they are loaded here, so that they are in flight while gs_krandom gathers its peers' status.
+      const bool whole = g.active_bytes <= g.udp_avail;
+      uint64_t tx8 = 0;
+      if (whole) {
+        uint32_t pm = queued;
+        for (uint32_t x = 0; x < 8u && pm != 0u; ++x) {
 #if defined(__CUDA_ARCH__)
           const uint32_t r = __ffs(pm) - 1;
 #else
           const uint32_t r = (uint32_t)__builtin_ctz(pm);
 #endif
           pm &= pm - 1;
+          tx8 |= (uint64_t)d.tx[GS_TX(r, cap, i)] << (8u * x);
+        }
+      }
+      uint32_t np = gs_krandom(d, g, i, t, GS_PUR_GOSSIP, kk, 0u, GS_EMPTY32, m, peers);
+      const uint32_t q0 = queued;
+      if (whole && np != 0u) {
+        // Broadcast r rides in packets 0 .. sends_r - 1 with sends_r = min(np, max(1, limit - transmits_r)):
+        // one read and one write of its counter instead of one per packet, same counters and same packets
+        // as the general loop below.  sends_r <= np <= 8: four bits each.
+        uint32_t sends = 0, n_pkts = 0, n_q = 0, pm = queued;
+        bool few = true;
+        while (pm) {
+          pm &= pm - 1;
           if (n_q == 8u) { few = false; break; }
-          const uint32_t tx = d.tx[GS_TX(r, cap, i)];
+          const uint32_t tx = (uint32_t)(tx8 >> (8u * n_q)) & 0xFFu;
           uint32_t room = g.retransmit_limit > tx ? g.retransmit_limit - tx : 1u;
           if (room == 0u) room = 1u;
           const uint32_t s = room < np ? room : np;
-          sends[n_q++] = s;
+          sends |= s << (4u * n_q++);
           if (s > n_pkts) n_pkts = s;
         }
         if (few) {
@@ -834,10 +849,11 @@ GS_DEV void gs_row_step_body(const GsDev& d, const GsGlobals& g, uint32_t i, uin
             const uint32_t r = (uint32_t)__builtin_ctz(pm);
 #endif
             pm &= pm - 1;
-            const uint32_t tx = (uint32_t)d.tx[GS_TX(r, cap, i)] + sends[x];
+            const uint32_t s = (sends >> (4u * x)) & 15u;
+            const uint32_t tx = ((uint32_t)(tx8 >> (8u * x)) & 0xFFu) + s;
             d.tx[GS_TX(r, cap, i)] = (uint8_t)tx;
             if (tx >= g.retransmit_limit) queued &= ~(1u << r);  // broadcast finished
-            sink.stat(GS_ST_RUMORS_SENT, sends[x]);
+            sink.stat(GS_ST_RUMORS_SENT, s);
           }
           sink.stat(GS_ST_GOSSIP_PACKETS, n_pkts);
           for (uint32_t q = 0; q < n_pkts; ++q) {
@@ -850,7 +866,7 @@ GS_DEV void gs_row_step_body(const GsDev& d, const GsGlobals& g, uint32_t i, uin
               const uint32_t r = (uint32_t)__builtin_ctz(pm);
 #endif
               pm &= pm - 1;
-              if (sends[x] > q) pkt |= 1u << r;
+              if (((sends >> (4u * x)) & 15u) > q) pkt |= 1u << r;
             }
             if (!gs_lost(g, imp_loss, sink, i, peers[q], t, GS_LK_GOSSIP, q))
               gs_post(d, g, sink, (t + 1u + gs_extra(g, imp_delay, i, peers[q])) & g.ring_mask, peers[q], pkt);
