@@ -158,6 +158,7 @@ SIGNATURES = [
     ("gsim_last_step_timing", _i32, [_P, C.POINTER(C.c_double), C.POINTER(_u64)]),
     ("gsim_launch_count", _u64, [_P]),
     ("gsim_sched_counts", _i32, [_P, C.POINTER(_u64)]),
+    ("gsim_piggyback_stats", _i32, [_P, C.POINTER(_u64)]),
     ("gsim_ring_entry", _u32, [_u64, _u32, _u32, _u32, _u32]),
     ("gsim_ring_position", _u32, [_u64, _u32, _u32, _u32, _u32]),
     ("gsim_wire_alive", _sz, [_P, _sz, _u32, C.c_char_p, _P, _sz, C.c_uint16, _P, _sz, C.POINTER(C.c_uint8)]),
@@ -168,6 +169,11 @@ SIGNATURES = [
     ("gsim_wire_user_event", _sz, [_P, _sz, _u64, _P, _sz, _P, _sz, _i32]),
     ("gsim_wire_compound", _sz, [_P, _sz, C.POINTER(_P), C.POINTER(_sz), _sz]),
     ("gsim_wire_wanfed_frame", _sz, [_P, _sz, _P, _sz]),
+    ("gsim_wire_ping", _sz, [_P, _sz, _u32, C.c_char_p, _P, _sz, C.c_uint16, C.c_char_p]),
+    ("gsim_wire_indirect_ping", _sz, [_P, _sz, _u32, _P, _sz, C.c_uint16, C.c_char_p, _i32, _P, _sz, C.c_uint16,
+                                      C.c_char_p]),
+    ("gsim_wire_ack", _sz, [_P, _sz, _u32, _P, _sz]),
+    ("gsim_wire_nack", _sz, [_P, _sz, _u32]),
     ("gsim_wire_consul_user_event", _sz, [_P, _sz, C.c_char_p, C.c_char_p, _P, _sz, C.c_char_p, C.c_char_p,
                                           C.c_char_p, _i32]),
 ]

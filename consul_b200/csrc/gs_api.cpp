@@ -607,6 +607,24 @@ static bool reset_qstate(gsim_pool* p) {
   return true;
 }
 
+// Bytes a probe message leaves to piggybacked broadcasts ([U] memberlist/net.go sendMsg: UDPBufferSize -
+// len(msg) - compoundHeaderOverhead), by GS_PIG_*.  The messages as memberlist's probeNode / handleIndirectPing
+// send them: IPv4 address, port 8301, the name of the pool's last member id, "node-<capacity - 1>", on both ends,
+// a sequence number past 2^16 (5 bytes, a member that has probed for a day), acks without a ping-delegate payload.
+static void pig_budgets(const gsim_pool* p, uint32_t out[4]) {
+  char name[32];
+  const int len = snprintf(name, sizeof(name), "node-%u", p->cfg.capacity ? p->cfg.capacity - 1u : 0u);
+  const uint8_t addr[4] = {10, 0, 0, 1};
+  const uint32_t seq = 0x10000u;
+  size_t msg[4];
+  msg[GS_PIG_PING] = gsw::ping(nullptr, 0, seq, name, (size_t)len, addr, 4, 8301, name, (size_t)len);
+  msg[GS_PIG_ACK] = gsw::ack(nullptr, 0, seq, nullptr, 0);
+  msg[GS_PIG_NACK] = gsw::nack(nullptr, 0, seq);
+  msg[GS_PIG_INDREQ] = gsw::indirect_ping(nullptr, 0, seq, addr, 4, 8301, name, (size_t)len, true, addr, 4, 8301, name,
+                                          (size_t)len);
+  for (int k = 0; k < 4; ++k) out[k] = p->g.udp_avail > msg[k] ? p->g.udp_avail - (uint32_t)msg[k] : 0u;
+}
+
 // Device-side initial state: empty columns, zeroed counters, the converged initial members.
 // On a sharded pool this runs on rank 0 only and reaches every GPU through the unified columns.
 static int init_device_state(gsim_pool* p) {
@@ -632,6 +650,12 @@ static int init_device_state(gsim_pool* p) {
         be->fill32(reinterpret_cast<uint32_t*>(d.acc), GS_EMPTY32, cap * GS_K1MAX * 2 * 2);
   okk = okk && be->fill8(d.tx, 0, cap * GS_MAX_RUMORS);
   if (d.ppreq) okk = okk && be->fill32(d.ppreq, GS_EMPTY32, cap * 2 * GS_PPK) && be->fill32(d.pp_clk, 0, cap * 4);
+  if (d.pig) {
+    GsPig pig;
+    memset(&pig, 0, sizeof(pig));
+    pig_budgets(p, pig.budget);
+    okk = okk && be->fill32(d.pig_req, GS_EMPTY32, cap * 2 * GS_PIGK) && be->h2d(d.pig, &pig, sizeof(pig));
+  }
   okk = okk && be->fill32(reinterpret_cast<uint32_t*>(d.stats), 0, GSIM_STAT_COUNT * 2);
   okk = okk && be->fill32(d.heard_cnt, 0, 32) && be->fill32(d.conv_tick, GS_EMPTY32, 32);
   okk = okk && be->fill32(d.view_cnt, 0, 4) && be->fill32(d.crashed_alive, 0, 1);
@@ -692,6 +716,12 @@ extern "C" int gsim_pool_create(const gsim_config* cfg, gsim_pool** out) {
   // mailbox ring: 2 arrival slots unless the pool is going to carry a latency matrix
   const uint32_t ring_depth = cfg->mailbox_depth ? cfg->mailbox_depth : 2u;
   if (ring_depth < 2 || ring_depth > GS_RING_MAX || (ring_depth & (ring_depth - 1u)) != 0) return GSIM_ERR_INVALID;
+
+  if (sharded && (cfg->flags & GSIM_FLAG_PROBE_PIGGYBACK)) {
+    g_create_err = "GSIM_FLAG_PROBE_PIGGYBACK is not supported on sharded pools";
+    fprintf(stderr, "libgsim: %s\n", g_create_err.c_str());
+    return GSIM_ERR_INVALID;
+  }
 
   char errbuf[256] = {0};
   GsBackend* be = GS_MAKE_BACKEND(cfg->device, errbuf, sizeof(errbuf));
@@ -784,6 +814,8 @@ extern "C" int gsim_pool_create(const gsim_config* cfg, gsim_pool** out) {
   }
   if (cfg->flags & GSIM_FLAG_PUSH_PULL)  // push-pull mailboxes: 48 B per member, only when asked for
     okk = okk && acol(&d.ppreq, 2 * GS_PPK) && acol(&d.pp_clk, 4);
+  if (cfg->flags & GSIM_FLAG_PROBE_PIGGYBACK)  // owed answers: 32 B per member, only when asked for
+    okk = okk && alloc_col(p, &d.pig_req, cap * 2 * GS_PIGK) && alloc_col(p, &d.pig, (size_t)1);
   uint32_t evcap = cfg->event_log_capacity ? cfg->event_log_capacity : 65536u;
   if (!sharded) {
     okk = okk && alloc_col(p, &d.stats, (size_t)GSIM_STAT_COUNT);
@@ -1079,7 +1111,9 @@ static int alloc_slot(gsim_pool* p, uint32_t* slot_out) {
 
 // A member whose broadcast queue became non-empty between ticks must be looked at by the
 // next tick: set the wake bit in the mailbox that tick will read.
+// A piggybacking pool also stamps its gate for that tick (GsPig::gate).
 static bool post_wake(gsim_pool* p, uint32_t row) {
+  if (p->d.pig && !poke(p, reinterpret_cast<uint32_t*>(p->d.pig), p->now % GS_PIG_GATES, p->now + 1u)) return false;
   return poke_or(p, p->d.inbox[p->now & p->g.ring_mask], row, GS_WAKE_BIT);
 }
 
@@ -2720,6 +2754,19 @@ static int advance_ticks(gsim_pool* p, uint32_t chunk, bool use_graph) {
   return GSIM_OK;
 }
 
+extern "C" int gsim_piggyback_stats(gsim_pool* p, uint64_t out[4]) {
+  if (!p || !out) return GSIM_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(p->mu);
+  if (!p->d.pig) return fail(p, GSIM_ERR_STATE, "the pool was created without GSIM_FLAG_PROBE_PIGGYBACK");
+  GsPig pig;
+  if (!flush_writes(p) || !dev(p)->d2h(&pig, p->d.pig, sizeof(pig))) return fail(p, GSIM_ERR_CUDA, "d2h");
+  for (int k = 0; k < 4; ++k) {
+    out[k] = 0;
+    for (int l = 0; l < 32; ++l) out[k] += pig.stats[k][l];
+  }
+  return GSIM_OK;
+}
+
 extern "C" int gsim_sched_counts(gsim_pool* p, uint64_t out[8]) {
   if (!p || !out) return GSIM_ERR_INVALID;
   std::lock_guard<std::mutex> lk(p->mu);
@@ -3203,6 +3250,10 @@ static std::vector<SnapCol> snap_cols(gsim_pool* p, bool with_impairment, bool w
     add(d.ppreq, cap * 4 * 2 * GS_PPK, 2 * GS_PPK);
     add(d.pp_clk, cap * 4 * 4, 4);
   }
+  if (d.pig) {
+    add(d.pig_req, cap * 4 * 2 * GS_PIGK, 2 * GS_PIGK);
+    add(d.pig, sizeof(GsPig), 1, false);
+  }
   if (with_impairment) {
     add(p->imp_loss, cap * 4);
     add(p->imp_delay, cap);
@@ -3243,6 +3294,7 @@ static uint32_t snap_layout(const gsim_pool* p) {
   if (p->sharded) m |= 16u;
   if (p->pause_until) m |= 32u;  // the pause column and statistics (restore allocates them when the pool has none)
   if (p->imp_recv) m |= 64u;     // the reachability columns (with bit 8; restore allocates them when the pool has none)
+  if (p->d.pig) m |= 128u;       // owed answers and the piggyback words (GSIM_FLAG_PROBE_PIGGYBACK)
   return m;
 }
 static uint64_t snap_graph_hash(const gsim_pool* p) {
@@ -3488,6 +3540,21 @@ extern "C" size_t gsim_wire_compound(void* out, size_t cap, const void* const* m
 extern "C" size_t gsim_wire_wanfed_frame(void* out, size_t cap, const void* packet, size_t len) {
   return gsw::wanfed_frame(out, cap, packet, len);
 }
+extern "C" size_t gsim_wire_ping(void* out, size_t cap, uint32_t seq_no, const char* node, const void* source_addr,
+                                 size_t source_addr_len, uint16_t source_port, const char* source_node) {
+  return gsw::ping(out, cap, seq_no, node, zlen(node), source_addr, source_addr_len, source_port, source_node,
+                   zlen(source_node));
+}
+extern "C" size_t gsim_wire_indirect_ping(void* out, size_t cap, uint32_t seq_no, const void* target, size_t target_len,
+                                          uint16_t port, const char* node, int nack, const void* source_addr,
+                                          size_t source_addr_len, uint16_t source_port, const char* source_node) {
+  return gsw::indirect_ping(out, cap, seq_no, target, target_len, port, node, zlen(node), nack != 0, source_addr,
+                            source_addr_len, source_port, source_node, zlen(source_node));
+}
+extern "C" size_t gsim_wire_ack(void* out, size_t cap, uint32_t seq_no, const void* payload, size_t payload_len) {
+  return gsw::ack(out, cap, seq_no, payload, payload_len);
+}
+extern "C" size_t gsim_wire_nack(void* out, size_t cap, uint32_t seq_no) { return gsw::nack(out, cap, seq_no); }
 extern "C" size_t gsim_wire_consul_user_event(void* out, size_t cap, const char* id, const char* name,
                                               const void* payload, size_t payload_len, const char* node_filter,
                                               const char* service_filter, const char* tag_filter, int version) {

@@ -207,6 +207,10 @@ GS_DEV uint64_t gs_hash_row(const GsDev& d, const GsGlobals& g, uint32_t i, uint
       h = gs_mix64(h, clk[i]);
       h = gs_mix64(h, clk[cap + i]);
     }
+    if (d.pig_req != nullptr) {  // probe-path answers this member owes (GSIM_FLAG_PROBE_PIGGYBACK)
+      const uint32_t* req = d.pig_req + (size_t)cur * GS_PIGK * cap;
+      for (uint32_t s = 0; s < GS_PIGK; ++s) h = gs_mix64(h, req[(size_t)s * cap + i]);
+    }
   }
   return h;
 }

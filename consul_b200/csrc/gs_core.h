@@ -408,6 +408,8 @@ struct GsEventRec {
   uint32_t tick, type, subject, observer, ltime, reserved;
 };
 
+struct GsPig;
+
 // Device column pointers.
 struct GsDev {
   uint32_t* key[2];      // the key column this rank READS (its own replica when sharded)
@@ -471,6 +473,29 @@ struct GsDev {
   // setting).  Last in the struct, so every other field keeps its offset.
   const uint32_t* imp_recv;
   const uint8_t* imp_flags;
+  // broadcasts piggybacked on probe traffic (GSIM_FLAG_PROBE_PIGGYBACK), both null without the flag:
+  // owed answers by arrival-tick parity, [2][GS_PIGK][cap] entries receiver << 3 | kind << 1 | lost, kept as
+  // the GS_PIGK smallest by an atomicMin chain; and the pool-wide words
+  uint32_t* pig_req;
+  GsPig* pig;
+};
+
+// Broadcasts piggybacked on probe traffic (GSIM_FLAG_PROBE_PIGGYBACK, DESIGN.md §3.7).
+#define GS_PIGK 4u       // owed answers one member serves per tick (smallest entries win), like GS_PPK
+#define GS_PIG_GATES 16u // gate words: tick s is gated iff gate[s % 16] == s + 1
+// The probe messages whose remaining UDP room carries broadcasts, and what an owed answer entry names.
+enum { GS_PIG_PING = 0, GS_PIG_ACK = 1, GS_PIG_NACK = 2, GS_PIG_INDREQ = 3 };
+// gsim_piggyback_stats counters
+enum { GS_PIG_ST_PACKETS = 0, GS_PIG_ST_BCASTS = 1, GS_PIG_ST_SERVED = 2, GS_PIG_ST_DROPPED = 3 };
+// Pool-wide words of a piggybacking pool (one device allocation, carried whole by snapshots).
+struct GsPig {
+  // "some member's broadcast queue was non-empty when tick s began" <=> gate[s % 16] == s + 1.  A row that
+  // ends tick t with a non-empty queue stamps every tick up to the one it is stepped at again (at most the
+  // mailbox ring depth, <= 8, ahead), the host stamps `now` when it queues something: the word a tick
+  // reads is never one that tick writes, and nobody has to clear a word.
+  uint32_t gate[GS_PIG_GATES];
+  uint32_t budget[4];                  // bytes left for broadcasts in a ping / ack / nack / indirect-ping request
+  unsigned long long stats[4][32];     // GS_PIG_ST_* per member id % 32 (summed on read)
 };
 
 // Pool-wide scheduling words (one copy per rank).  A pool is QUIET when every mailbox slot is empty

@@ -179,6 +179,13 @@ __device__ __noinline__ void gs_row_step_impaired_call(const GsDev* dp, const Gs
   DevSinkT<COORDS> sink{s_stat, s_heard, s_q};
   gs_row_step_body<true>(*dp, *gp, i, t, t % gp->GI, inb, sink);
 }
+// Pools that piggyback broadcasts on probe traffic (GSIM_FLAG_PROBE_PIGGYBACK) likewise.
+template <bool COORDS, bool IMPAIRED>
+__device__ __noinline__ void gs_row_step_pig_call(const GsDev* dp, const GsGlobals* gp, uint32_t i, uint32_t t,
+                                                  uint32_t inb, uint32_t* s_stat, uint32_t* s_heard, uint32_t* s_q) {
+  DevSinkT<COORDS> sink{s_stat, s_heard, s_q};
+  gs_row_step_body<IMPAIRED, true>(*dp, *gp, i, t, t % gp->GI, inb, sink);
+}
 template <bool COORDS>
 __device__ __noinline__ void gs_row_step_call(const GsDev* dp, const GsGlobals* gp, uint32_t i, uint32_t t,
                                               uint32_t inb, uint32_t* s_stat, uint32_t* s_heard, uint32_t* s_q) {
@@ -188,6 +195,16 @@ __device__ __noinline__ void gs_row_step_call(const GsDev* dp, const GsGlobals* 
   }
   DevSinkT<COORDS> sink{s_stat, s_heard, s_q};
   gs_row_step_body<false>(*dp, *gp, i, t, t % gp->GI, inb, sink);
+}
+
+// Every generic row step of the tick and window kernels: piggybacking pools call their own step from here, not
+// from inside gs_row_step_call, so that its frame does not stack on top of the default step's.
+template <bool COORDS>
+__device__ __forceinline__ void gs_row_step_any(const GsDev* dp, const GsGlobals* gp, uint32_t i, uint32_t t,
+                                                uint32_t inb, uint32_t* s_stat, uint32_t* s_heard, uint32_t* s_q) {
+  if (dp->pig == nullptr) gs_row_step_call<COORDS>(dp, gp, i, t, inb, s_stat, s_heard, s_q);
+  else if (dp->imp_loss != nullptr) gs_row_step_pig_call<COORDS, true>(dp, gp, i, t, inb, s_stat, s_heard, s_q);
+  else gs_row_step_pig_call<COORDS, false>(dp, gp, i, t, inb, s_stat, s_heard, s_q);
 }
 
 // Tick stretches (run_tick_stretch): the control block on the device, in the backend's scratch.
@@ -461,7 +478,7 @@ __global__ void __launch_bounds__(GS_BLOCK, GS_MIN_BLOCKS)
     if (idx + lane < n_work) {
       const uint32_t e = s_work[idx + lane];
       const uint32_t i = (s_rtile[e >> 9] + ((e >> 7) & 3u)) * GS_TILE + (e & 127u);
-      gs_row_step_call<COORDS>(&d, gp, i, t, __ldcg(inbox_cur + i), s_stat, s_heard, s_q);
+      gs_row_step_any<COORDS>(&d, gp, i, t, __ldcg(inbox_cur + i), s_stat, s_heard, s_q);
     }
   }
   __syncthreads();  // the queue is drained (and its counters may be reused two rounds from now)
@@ -585,7 +602,7 @@ __device__ __noinline__ void gs_window_generic(const GsDev* dp, const GsGlobals*
           const uint32_t t = which == 0 ? (a < b ? a : b) : (a < b ? b : a);
           if (t >= w1) break;
           // (a member the fast path finished at `a` has moved its `due` on: it is not stepped twice)
-          if (sl && __ldcg(d.due + i) == t) gs_row_step_call<COORDS>(&d, gp, i, t, 0u, s_stat, s_heard, s_q);
+          if (sl && __ldcg(d.due + i) == t) gs_row_step_any<COORDS>(&d, gp, i, t, 0u, s_stat, s_heard, s_q);
         }
       }
     }

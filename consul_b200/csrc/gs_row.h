@@ -382,10 +382,12 @@ GS_DEV uint32_t gs_krandom(const GsDev& d, const GsGlobals& g, uint32_t i, uint3
 
 // TransmitLimitedQueue.GetBroadcasts ([U] memberlist/queue.go) for one packet: walk the
 // member's queued rumors by (queue class, transmits asc, size desc, slot desc) and take
-// every message that still fits the UDP budget.  Class order = memberlist broadcasts,
+// every message that still fits `avail` bytes: UDPBufferSize - compoundHeaderOverhead for a gossip
+// packet (gs_select_packet), what the probe message leaves for one that rides on probe traffic
+// ([U] memberlist/net.go sendMsg -> getBroadcasts, gs_pig_take).  Class order = memberlist broadcasts,
 // then serf intents, then serf user events ([U] serf/delegate.go GetBroadcasts).
-GS_DEV uint32_t gs_select_packet(const GsDev& d, const GsGlobals& g, uint32_t i, uint32_t queued) {
-  if (g.active_bytes <= g.udp_avail) return queued;  // every tracked broadcast together fits one packet
+GS_DEV uint32_t gs_select_packet_in(const GsDev& d, const GsGlobals& g, uint32_t i, uint32_t queued, uint32_t avail) {
+  if (g.active_bytes <= avail) return queued;
   uint32_t total = 0, qm = queued;
   while (qm) {
 #if defined(__CUDA_ARCH__)
@@ -396,14 +398,14 @@ GS_DEV uint32_t gs_select_packet(const GsDev& d, const GsGlobals& g, uint32_t i,
     qm &= qm - 1;
     total += g.rumors[r].size + (g.rumors[r].qclass ? 3u : 2u);
   }
-  if (total <= g.udp_avail) return queued;  // everything fits: the common case
+  if (total <= avail) return queued;
   uint32_t used = 0, mask = 0;
   for (uint32_t cls = 0; cls < 3; ++cls) {
     uint32_t cm = queued & g.class_mask[cls];
     const uint32_t ovh = cls ? 3u : 2u;
     while (cm) {
-      if (g.udp_avail <= used + ovh) break;
-      const uint32_t free_b = g.udp_avail - used - ovh;
+      if (avail <= used + ovh) break;
+      const uint32_t free_b = avail - used - ovh;
       uint32_t best = GS_EMPTY32, best_key = GS_EMPTY32, scan = cm;
       while (scan) {
 #if defined(__CUDA_ARCH__)
@@ -428,6 +430,87 @@ GS_DEV uint32_t gs_select_packet(const GsDev& d, const GsGlobals& g, uint32_t i,
     }
   }
   return mask;
+}
+
+GS_DEV uint32_t gs_select_packet(const GsDev& d, const GsGlobals& g, uint32_t i, uint32_t queued) {
+  return gs_select_packet_in(d, g, i, queued, g.udp_avail);
+}
+
+// ---- broadcasts piggybacked on probe traffic (GSIM_FLAG_PROBE_PIGGYBACK, DESIGN.md §3.7) ------------
+// Piggyback counters (GS_PIG_ST_*), one lane per member id % 32 so that a tick's many adds do not all meet
+// at one address; the host sums the lanes.
+GS_DEV void gs_pig_count(const GsDev& d, uint32_t i, uint32_t which, uint32_t v) {
+#if defined(__CUDA_ARCH__)
+  atomicAdd(&d.pig->stats[which][i & 31u], (unsigned long long)v);
+#else
+  __atomic_fetch_add(&d.pig->stats[which][i & 31u], (unsigned long long)v, __ATOMIC_RELAXED);
+#endif
+}
+
+// Was some member's queue non-empty when tick t began (GsPig::gate)?  A member that sees a stale copy of the
+// word in a cache only re-stamps it with the value it already holds.
+GS_DEV bool gs_pig_gate(const GsDev& d, uint32_t t) { return d.pig->gate[t % GS_PIG_GATES] == t + 1u; }
+
+// Member whose queue is still non-empty at the end of tick t and is stepped again at t + delta at the latest.
+GS_DEV void gs_pig_stamp(const GsDev& d, uint32_t t, uint32_t delta) {
+  for (uint32_t s = t + 1u; s != t + 1u + delta; ++s)
+    if (d.pig->gate[s % GS_PIG_GATES] != s + 1u) d.pig->gate[s % GS_PIG_GATES] = s + 1u;
+}
+
+// The tick after t at which a member with a queue is stepped for it (gs_queue_wake_slot), as a distance.
+GS_DEV uint32_t gs_pig_wake_delta(const GsGlobals& g, uint32_t gslot, uint32_t gphase) {
+  const uint32_t next = gslot + 1u == g.GI ? 0u : gslot + 1u;
+  const uint32_t delta = (gphase >= next ? gphase - next : gphase + g.GI - next) + 1u;
+  return delta > g.ring_mask + 1u ? 1u : delta;
+}
+
+// One probe-path message of member i that carries broadcasts: a packet of its queue within the message's
+// budget, counted like a gossip packet (transmits + 1 whether or not it arrives, retired at the limit).
+// Returns the packet, 0 when nothing is queued or nothing fits (then nothing is sent or counted).
+GS_DEV uint32_t gs_pig_take(const GsDev& d, const GsGlobals& g, uint32_t i, uint32_t& queued, uint32_t kind) {
+  if (queued == 0u) return 0u;
+  const uint32_t pkt = gs_select_packet_in(d, g, i, queued, d.pig->budget[kind]);
+  if (pkt == 0u) return 0u;
+  const uint32_t q0 = queued;
+  uint32_t pm = pkt, c = 0;
+  while (pm) {
+#if defined(__CUDA_ARCH__)
+    const uint32_t r = __ffs(pm) - 1;
+#else
+    const uint32_t r = (uint32_t)__builtin_ctz(pm);
+#endif
+    pm &= pm - 1;
+    const uint32_t tx = (uint32_t)d.tx[GS_TX(r, g.cap, i)] + 1u;
+    d.tx[GS_TX(r, g.cap, i)] = (uint8_t)tx;
+    if (tx >= g.retransmit_limit) queued &= ~(1u << r);  // broadcast finished
+    ++c;
+  }
+  if (queued != q0) d.queued[i] = queued;
+  gs_pig_count(d, i, GS_PIG_ST_PACKETS, 1u);
+  gs_pig_count(d, i, GS_PIG_ST_BCASTS, c);
+  return pkt;
+}
+
+// A probe-path message that member `sender` owes `receiver` (an ack, a relay's ping, a nack): posted at tick
+// t, served by the sender in its own step at t + 1 (only a row writes its own queue).  Kept as the GS_PIGK
+// smallest entries by an atomicMin chain: every post either fills an empty slot or pushes exactly one entry
+// off the end, so which entries stay and how many are dropped do not depend on the order of the posts.
+template <class Sink>
+GS_DEV void gs_pig_owe(const GsDev& d, const GsGlobals& g, Sink& sink, uint32_t nxt, uint32_t inxt, uint32_t sender,
+                       uint32_t receiver, uint32_t kind, bool lost) {
+  uint32_t* req = d.pig_req + (size_t)nxt * GS_PIGK * g.cap;
+  uint32_t v = (receiver << 3) | (kind << 1) | (lost ? 1u : 0u);
+  bool kept = false;
+  for (uint32_t s = 0; s < GS_PIGK; ++s) {
+    const uint32_t old = GS_ATOMIC_MIN32(&req[(size_t)s * g.cap + sender], v);
+    if (old == GS_EMPTY32) {
+      kept = true;
+      break;
+    }
+    if (old > v) v = old;  // displaced a larger entry: carry it to the next slot (an equal one carries itself)
+  }
+  if (!kept) gs_pig_count(d, sender, GS_PIG_ST_DROPPED, 1u);
+  gs_post(d, g, sink, inxt, sender, GS_ACC_BIT);
 }
 
 template <class Sink>
@@ -479,7 +562,9 @@ GS_DEV bool gs_mail_is_stale(const GsGlobals& g, uint32_t w, uint32_t heard, boo
 // IMPAIRED: the pool has degraded members (GsDev::imp_loss / imp_recv / imp_delay are set, imp_flags
 // when some member has a directional setting).  The other instantiation folds every impairment term
 // away, so a pool without any runs the code it would run without the feature.
-template <bool IMPAIRED, class Sink>
+// PIG: the pool piggybacks broadcasts on probe traffic (GsDev::pig_req / pig are set); likewise folded away
+// in the other instantiation.
+template <bool IMPAIRED, bool PIG = false, class Sink>
 GS_DEV void gs_row_step_body(const GsDev& d, const GsGlobals& g, uint32_t i, uint32_t t, uint32_t gslot,
                              uint32_t inb, Sink& sink) {
   const GsLossCols imp_loss = {IMPAIRED ? d.imp_loss : nullptr, IMPAIRED ? d.imp_recv : nullptr};
@@ -520,6 +605,9 @@ GS_DEV void gs_row_step_body(const GsDev& d, const GsGlobals& g, uint32_t i, uin
       d.meta[i] = m0 & ~GS_META_DIRTY;
     }
     if (queued != 0u) gs_post(d, g, sink, gs_queue_wake_slot(g, t, gslot, gs_meta_gphase(m0)), i, GS_WAKE_BIT);
+    if constexpr (PIG) {
+      if (queued != 0u) gs_pig_stamp(d, t, gs_pig_wake_delta(g, gslot, gs_meta_gphase(m0)));
+    }
     return;
   }
 
@@ -639,6 +727,23 @@ GS_DEV void gs_row_step_body(const GsDev& d, const GsGlobals& g, uint32_t i, uin
         gs_post(d, g, sink, inxt, from, (d.heard[i] & g.active_mask) | GS_ACC_BIT);
       }
     }
+    if constexpr (PIG) {
+      if (inb & GS_ACC_BIT) {
+        // the probe-path messages this member owes since tick t - 1 (gs_pig_owe): each takes a packet of the
+        // queue as it is now and arrives one tick (plus latency) later unless its loss draw at t - 1 said lost
+        uint32_t* req = d.pig_req + (size_t)cur * GS_PIGK * cap;
+        for (uint32_t s = 0; s < GS_PIGK; ++s) {
+          const uint32_t e = GS_LD_OTHER(&req[(size_t)s * cap + i]);
+          if (e == GS_EMPTY32) break;
+          req[(size_t)s * cap + i] = GS_EMPTY32;
+          if (!up) continue;  // a process that is not running answers nothing
+          gs_pig_count(d, i, GS_PIG_ST_SERVED, 1u);
+          const uint32_t pkt = gs_pig_take(d, g, i, queued, (e >> 1) & 3u);
+          if (pkt != 0u && !(e & 1u))
+            gs_post(d, g, sink, (t + 1u + gs_extra(g, imp_delay, i, e >> 3)) & g.ring_mask, e >> 3, pkt);
+        }
+      }
+    }
   }
 
   // ---- B. the member's own view transitions -------------------------------------
@@ -687,10 +792,31 @@ GS_DEV void gs_row_step_body(const GsDev& d, const GsGlobals& g, uint32_t i, uin
       // Latency pools: whatever comes back must arrive before the probe deadline, i.e. within
       // `budget` ticks of extra latency from now (t0 + P*(awareness+1) - (t0 + T)).
       const uint32_t budget = g.P * (gs_meta_aw(m) + 1u) - g.T;
+      bool pig_gate = false;
+      if constexpr (PIG) pig_gate = gs_pig_gate(d, t);
       for (uint32_t q = 0; q < nr; ++q) {
         const uint32_t r = relays[q];
         const bool r_up = gs_key_truth(gs_peer_key(d, cur, r, false)) == GS_TRUTH_UP;
         sink.stat(GS_ST_INDIRECT_PINGS, 1);
+        if constexpr (PIG) {
+          // the request carries broadcasts of this member's queue; the relay's ping to j, j's ack and the
+          // relay's forwarded ack or nack are owed by whoever sends them (same loss draws as below)
+          const bool req_lost = gs_lost_quiet(g, imp_loss, i, r, t, GS_LK_INDREQ, q);
+          const uint32_t pkt = gs_pig_take(d, g, i, queued, GS_PIG_INDREQ);
+          if (pkt != 0u && !req_lost) gs_post(d, g, sink, (t + 1u + gs_extra(g, imp_delay, i, r)) & g.ring_mask, r, pkt);
+          if (pig_gate && r_up && !req_lost) {
+            const bool ping_lost = gs_lost_quiet(g, imp_loss, r, j, t, GS_LK_INDPING, q);
+            gs_pig_owe(d, g, sink, nxt, inxt, r, j, GS_PIG_PING, ping_lost);
+            const bool ack_lost = gs_lost_quiet(g, imp_loss, j, r, t, GS_LK_INDACK, q);
+            if (j_up && !ping_lost) gs_pig_owe(d, g, sink, nxt, inxt, j, r, GS_PIG_ACK, ack_lost);
+            const bool acked = j_up && !ping_lost && !ack_lost &&
+                               gs_extra(g, imp_delay, r, j) + gs_extra(g, imp_delay, j, r) <= g.T;
+            if (acked)
+              gs_pig_owe(d, g, sink, nxt, inxt, r, i, GS_PIG_ACK, gs_lost_quiet(g, imp_loss, r, i, t, GS_LK_INDFWD, q));
+            else
+              gs_pig_owe(d, g, sink, nxt, inxt, r, i, GS_PIG_NACK, gs_lost_quiet(g, imp_loss, r, i, t, GS_LK_NACK, q));
+          }
+        }
         if (!(r_up && !gs_lost(g, imp_loss, sink, i, r, t, GS_LK_INDREQ, q))) continue;  // no nack either
         const uint32_t via = gs_extra(g, imp_delay, i, r) + gs_extra(g, imp_delay, r, i);
         const uint32_t rtt_rj = gs_extra(g, imp_delay, r, j) + gs_extra(g, imp_delay, j, r);
@@ -778,6 +904,15 @@ GS_DEV void gs_row_step_body(const GsDev& d, const GsGlobals& g, uint32_t i, uin
       d.pass[i] = pass;
       if (target != GS_EMPTY32) {
         sink.stat(GS_ST_PROBES, 1);
+        if constexpr (PIG) {
+          // the ping carries broadcasts of this member's queue; the target owes its ack (same loss draws as below)
+          const bool ping_lost = gs_lost_quiet(g, imp_loss, i, target, t, GS_LK_PING, 0);
+          const uint32_t pkt = gs_pig_take(d, g, i, queued, GS_PIG_PING);
+          if (pkt != 0u && !ping_lost)
+            gs_post(d, g, sink, (t + 1u + gs_extra(g, imp_delay, i, target)) & g.ring_mask, target, pkt);
+          if (gs_pig_gate(d, t) && gs_key_truth(ktarget) == GS_TRUTH_UP && !ping_lost)
+            gs_pig_owe(d, g, sink, nxt, inxt, target, i, GS_PIG_ACK, gs_lost_quiet(g, imp_loss, target, i, t, GS_LK_ACK, 0));
+        }
         bool ok = gs_key_truth(ktarget) == GS_TRUTH_UP && !gs_lost(g, imp_loss, sink, i, target, t, GS_LK_PING, 0) &&
                   !gs_lost(g, imp_loss, sink, target, i, t, GS_LK_ACK, 0) &&
                   gs_extra(g, imp_delay, i, target) + gs_extra(g, imp_delay, target, i) <= g.T;  // ack within ProbeTimeout
@@ -941,11 +1076,21 @@ GS_DEV void gs_row_step_body(const GsDev& d, const GsGlobals& g, uint32_t i, uin
     gs_post(d, g, sink, inxt, i, GS_WAKE_BIT);
   else if (queued != 0u)
     gs_post(d, g, sink, gs_queue_wake_slot(g, t, gslot, gs_meta_gphase(m)), i, GS_WAKE_BIT);
+  if constexpr (PIG) {
+    if (queued != 0u)
+      gs_pig_stamp(d, t, gs_key_rank(k) == GS_RANK_SUSPECT || (m & GS_META_DIRTY) ? 1u
+                                                                                    : gs_pig_wake_delta(g, gslot, gs_meta_gphase(m)));
+  }
 }
 
 template <class Sink>
 GS_DEV void gs_row_step(const GsDev& d, const GsGlobals& g, uint32_t i, uint32_t t, uint32_t gslot, uint32_t inb,
                         Sink& sink) {
+  if (d.pig != nullptr) {
+    if (d.imp_loss != nullptr) gs_row_step_body<true, true>(d, g, i, t, gslot, inb, sink);
+    else gs_row_step_body<false, true>(d, g, i, t, gslot, inb, sink);
+    return;
+  }
   if (d.imp_loss != nullptr) gs_row_step_body<true>(d, g, i, t, gslot, inb, sink);
   else gs_row_step_body<false>(d, g, i, t, gslot, inb, sink);
 }
@@ -996,6 +1141,9 @@ GS_DEV bool gs_fast_finish(const GsDev& d, const G& g, Sink& sink, uint32_t i, u
     return false;  // ring entry must be skipped or needs the heard mask: generic path
   if (g.pp_interval != 0u && gs_pp_due(g.pp_interval, g.rot_pp, i / g.phase_group, t))
     return false;  // the push-pull ticker fires too: generic path
+  // piggybacking pool while some queue is non-empty: the probe may carry broadcasts or owe an ack's (every
+  // queue is empty while the gate is clear, the prober's own included)
+  if (d.pig != nullptr && gs_pig_gate(d, t)) return false;
   uint32_t m = f.m;
   if (gs_key_truth(f.kc) == GS_TRUTH_UP && gs_extra(g, nullptr, i, f.c) + gs_extra(g, nullptr, f.c, i) <= g.T) {
     const uint32_t aw = gs_meta_aw(m);

@@ -104,6 +104,59 @@ inline size_t suspect_or_dead(void* out, size_t cap, bool dead, uint32_t inc, co
   mp_key(b, "From"); mp_str(b, from, from_len, false);
   return b.n;
 }
+// Probe messages ([U] memberlist/net.go).  ping{SeqNo uint32; Node string; SourceAddr []byte; SourcePort
+// uint16; SourceNode string}, the three source fields `codec:",omitempty"`.
+inline void probe_source(Buf& b, const void* addr, size_t addr_len, uint16_t port, const char* src, size_t src_len) {
+  if (addr != nullptr && addr_len) { mp_key(b, "SourceAddr"); mp_bytes(b, addr, addr_len, false); }
+  if (port) { mp_key(b, "SourcePort"); mp_uint(b, port); }
+  if (src_len) { mp_key(b, "SourceNode"); mp_str(b, src, src_len, false); }
+}
+inline uint32_t probe_source_fields(const void* addr, size_t addr_len, uint16_t port, size_t src_len) {
+  return (addr != nullptr && addr_len ? 1u : 0u) + (port ? 1u : 0u) + (src_len ? 1u : 0u);
+}
+inline size_t ping(void* out, size_t cap, uint32_t seq, const char* node, size_t node_len, const void* addr,
+                   size_t addr_len, uint16_t port, const char* src, size_t src_len) {
+  Buf b(out, cap);
+  b.put(ML_PING);
+  mp_map(b, 2 + probe_source_fields(addr, addr_len, port, src_len));
+  mp_key(b, "SeqNo"); mp_uint(b, seq);
+  mp_key(b, "Node"); mp_str(b, node, node_len, false);
+  probe_source(b, addr, addr_len, port, src, src_len);
+  return b.n;
+}
+// indirectPingReq{SeqNo uint32; Target []byte; Port uint16; Node string; Nack bool; SourceAddr; SourcePort;
+// SourceNode}, the source fields omitempty
+inline size_t indirect_ping(void* out, size_t cap, uint32_t seq, const void* target, size_t target_len, uint16_t port,
+                            const char* node, size_t node_len, bool nack, const void* addr, size_t addr_len,
+                            uint16_t src_port, const char* src, size_t src_len) {
+  Buf b(out, cap);
+  b.put(ML_INDIRECT_PING);
+  mp_map(b, 5 + probe_source_fields(addr, addr_len, src_port, src_len));
+  mp_key(b, "SeqNo"); mp_uint(b, seq);
+  mp_key(b, "Target"); mp_bytes(b, target, target_len, false);
+  mp_key(b, "Port"); mp_uint(b, port);
+  mp_key(b, "Node"); mp_str(b, node, node_len, false);
+  mp_key(b, "Nack"); mp_bool(b, nack);
+  probe_source(b, addr, addr_len, src_port, src, src_len);
+  return b.n;
+}
+// ackResp{SeqNo uint32; Payload []byte} and nackResp{SeqNo uint32}
+inline size_t ack(void* out, size_t cap, uint32_t seq, const void* payload, size_t payload_len) {
+  Buf b(out, cap);
+  b.put(ML_ACK);
+  mp_map(b, 2);
+  mp_key(b, "SeqNo"); mp_uint(b, seq);
+  mp_key(b, "Payload"); mp_bytes(b, payload, payload_len, false);
+  return b.n;
+}
+inline size_t nack(void* out, size_t cap, uint32_t seq) {
+  Buf b(out, cap);
+  b.put(ML_NACK);
+  mp_map(b, 1);
+  mp_key(b, "SeqNo"); mp_uint(b, seq);
+  return b.n;
+}
+
 // [U] memberlist/util.go makeCompoundMessage
 inline size_t compound(void* out, size_t cap, const void* const* msgs, const size_t* lens, size_t count) {
   Buf b(out, cap);

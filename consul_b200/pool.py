@@ -25,6 +25,7 @@ FLAG_NO_GRAPH = 2
 FLAG_NO_WINDOWS = 16
 FLAG_PUSH_PULL = 32
 FLAG_COORDINATES = 64
+FLAG_PROBE_PIGGYBACK = 256  # broadcasts ride on pings, acks, indirect pings and nacks (DESIGN.md 3.7)
 MEMBER_WATCHED = 1
 MAX_DCS = 64  # datacenters of a latency matrix
 
@@ -417,6 +418,13 @@ class Pool:
         return {"window_launches": int(out[0]), "window_ticks": int(out[1]), "tick_launches": int(out[2]),
                 "horizon_scans": int(out[3]), "window_ms": out[4] / 1e6, "tick_ms": out[5] / 1e6,
                 "closed_form_launches": int(out[6]), "closed_form_ticks": int(out[7])}
+
+    def piggyback_stats(self) -> dict:
+        """Probe traffic that carried broadcasts (pools created with FLAG_PROBE_PIGGYBACK)."""
+        out = (C.c_uint64 * 4)()
+        self._ck(self.lib.gsim_piggyback_stats(self.h, out))
+        return {"packets": int(out[0]), "broadcasts": int(out[1]), "owed_served": int(out[2]),
+                "owed_dropped": int(out[3])}
 
     def launch_count(self) -> int:
         return int(self.lib.gsim_launch_count(self.h))

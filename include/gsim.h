@@ -159,6 +159,13 @@ typedef struct gsim_config {
  * trip (0.5 ms + the latency matrix there and back) and the target's coordinate.  348 B per
  * member; single-GPU pools.  IEEE double arithmetic, bit-identical to the oracle. */
 #define GSIM_FLAG_COORDINATES 64u
+/* Piggyback queued broadcasts on probe traffic ([U] memberlist/net.go sendMsg -> getBroadcasts;
+ * DESIGN.md 3.7): a ping and an indirect-ping request carry what room their packet leaves from the
+ * prober's queue, and acks, a relay's ping, forwarded acks and nacks carry the sender's, served one tick
+ * after the probe.  Every broadcast they carry counts as a transmission, as in a gossip packet.  Off by
+ * default: a pool without it runs exactly what it ran before.  Single-GPU pools (create fails on a
+ * sharded one, see gsim_last_error). */
+#define GSIM_FLAG_PROBE_PIGGYBACK 256u
 
 /* Preset defaults.  LAN/WAN: [U] memberlist DefaultLANConfig/DefaultWANConfig as
  * pinned by agent/config/runtime.go:1271-1413 with Consul's overrides
@@ -481,6 +488,12 @@ typedef struct gsim_stats {
   uint32_t events_dropped;
 } gsim_stats;
 int gsim_stats_get(gsim_pool* p, gsim_stats* out);
+/* Probe traffic that carried broadcasts (GSIM_FLAG_PROBE_PIGGYBACK) since creation: out[0] = probe-path
+ * messages that carried at least one broadcast, out[1] = broadcasts they carried (transmissions, on top of
+ * GSIM_STAT_RUMORS_SENT, which counts gossip packets only), out[2] = owed answers (acks, relay pings,
+ * forwarded acks, nacks) served by a running member, out[3] = owed answers dropped because their sender
+ * already owed 4 with smaller entries in that tick.  GSIM_ERR_STATE on a pool without the flag. */
+int gsim_piggyback_stats(gsim_pool* p, uint64_t out[4]);
 
 /* Order-independent 4x64-bit digest of the complete integer state (SURVEY 8d/8e:
  * equal for GPU and oracle, and for every shard count G). */
@@ -549,6 +562,15 @@ size_t gsim_wire_user_event(void* out, size_t cap, uint64_t ltime, const void* n
 /* memberlist compound packet of `count` messages (count <= 255) */
 size_t gsim_wire_compound(void* out, size_t cap, const void* const* msgs, const size_t* lens, size_t count);
 size_t gsim_wire_wanfed_frame(void* out, size_t cap, const void* packet, size_t len);
+/* memberlist's probe messages (net.go ping / indirectPingReq / ackResp / nackResp behind their type byte).
+ * Empty source fields are omitted (codec omitempty); a NULL payload is msgpack nil. */
+size_t gsim_wire_ping(void* out, size_t cap, uint32_t seq_no, const char* node, const void* source_addr,
+                      size_t source_addr_len, uint16_t source_port, const char* source_node);
+size_t gsim_wire_indirect_ping(void* out, size_t cap, uint32_t seq_no, const void* target, size_t target_len,
+                               uint16_t port, const char* node, int nack, const void* source_addr,
+                               size_t source_addr_len, uint16_t source_port, const char* source_node);
+size_t gsim_wire_ack(void* out, size_t cap, uint32_t seq_no, const void* payload, size_t payload_len);
+size_t gsim_wire_nack(void* out, size_t cap, uint32_t seq_no);
 size_t gsim_wire_consul_user_event(void* out, size_t cap, const char* id, const char* name, const void* payload,
                                    size_t payload_len, const char* node_filter, const char* service_filter,
                                    const char* tag_filter, int version);

@@ -121,6 +121,12 @@ class Pool {
     c.phase_group = 1;
     return c;
   }
+  // memberlist piggybacks queued broadcasts on pings, acks, indirect pings and nacks ([U] net.go sendMsg); the
+  // simulation does so for pools created from a config passed through here (GSIM_FLAG_PROBE_PIGGYBACK, off by default).
+  static gsim_config WithProbePiggyback(gsim_config c, bool on = true) {
+    c.flags = on ? (c.flags | GSIM_FLAG_PROBE_PIGGYBACK) : (c.flags & ~GSIM_FLAG_PROBE_PIGGYBACK);
+    return c;
+  }
 
   void Step(uint32_t ticks) { check(gsim_step(h_, ticks)); }
   uint32_t Now() const { return gsim_now(h_); }
