@@ -72,6 +72,11 @@ class GsimRumorInfo(C.Structure):
         "heard_count", "converged_tick", "queued_count")]
 
 
+# gsim_agent_stats, in order (every field a uint32_t)
+AGENT_STATS_FIELDS = ("members", "failed", "left", "health_score", "member_time", "event_time", "query_time",
+                      "intent_queue", "event_queue", "query_queue", "memberlist_queue", "running")
+
+
 class GsimStats(C.Structure):
     _fields_ = [
         ("counters", C.c_uint64 * GSIM_STAT_COUNT), ("node_ticks", C.c_uint64),
@@ -142,6 +147,8 @@ SIGNATURES = [
     ("gsim_now", _u32, [_P]),
     ("gsim_members", _i32, [_P, _u32, C.POINTER(GsimMember), _sz, C.POINTER(_sz)]),
     ("gsim_num_nodes", _i32, [_P, _u32, C.POINTER(_u32)]),
+    ("gsim_agent_stats_read", _i32, [_P, _u32, _u32, _P]),
+    ("gsim_health_histogram", _i32, [_P, C.POINTER(_u64)]),
     ("gsim_poll_events", _i32, [_P, C.POINTER(GsimEvent), _sz, C.POINTER(_sz)]),
     ("gsim_rumor_info_get", _i32, [_P, _u32, C.POINTER(GsimRumorInfo)]),
     ("gsim_rumor_retire", _i32, [_P, _u32]),

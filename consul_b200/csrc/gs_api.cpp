@@ -2993,6 +2993,79 @@ extern "C" int gsim_num_nodes(gsim_pool* p, uint32_t observer, uint32_t* n) {
   });
 }
 
+// ---- per-agent observation (DESIGN.md §3.8, gs_agent.h) ---------------------------------------------
+static_assert(sizeof(GsAgentStats) == sizeof(gsim_agent_stats), "GsAgentStats is gsim_agent_stats field for field");
+
+bool GsBackend::agent_stats(const GsDev& d, const GsGlobals& g, const uint32_t* key, const GsPendingAlive& pa,
+                            uint32_t first, uint32_t count, GsAgentStats* out) {
+  const size_t n = g.n;
+  std::vector<uint32_t> k(n), meta(n), heard(n), queued(n), lm(n), le(n), rp, col;
+  if (!d2h(k.data(), key, n * 4) || !d2h(meta.data(), d.meta, n * 4) || !d2h(heard.data(), d.heard, n * 4) ||
+      !d2h(queued.data(), d.queued, n * 4) || !d2h(lm.data(), d.ltime_member, n * 4) ||
+      !d2h(le.data(), d.ltime_event, n * 4))
+    return false;
+  uint32_t est[4] = {0u, 0u, 0u, 0u};
+  if (g.graph_n) {
+    rp.resize(n + 1);
+    if (!d2h(rp.data(), d.row_ptr, (n + 1) * 4)) return false;
+    col.resize(rp[n]);
+    if (rp[n] && !d2h(col.data(), d.col_idx, (size_t)rp[n] * 4)) return false;
+  } else {
+    for (size_t i = 0; i < n; ++i)
+      if (const uint32_t r1 = gs_established_rank1(k[i])) est[r1 - 1u]++;
+  }
+  const GsAgentCols c = {k.data(), meta.data(), heard.data(), queued.data(), lm.data(), le.data(),
+                         g.graph_n ? rp.data() : nullptr, g.graph_n ? col.data() : nullptr};
+  for (uint32_t x = 0; x < count; ++x) out[x] = gs_agent_stats_row(c, g.class_mask, est, pa, first + x);
+  return true;
+}
+
+bool GsBackend::health_histogram(const GsDev& d, const GsGlobals& g, const uint32_t* key, const GsImpairCols& imp,
+                                 uint64_t out[GS_HIST_BINS]) {
+  const size_t n = g.n;
+  for (uint32_t b = 0; b < GS_HIST_BINS; ++b) out[b] = 0u;
+  std::vector<uint32_t> k(n), meta(n), loss(imp.loss ? n : 0u), recv(imp.recv ? n : 0u);
+  std::vector<uint8_t> delay(imp.delay ? n : 0u), flags(imp.flags ? n : 0u);
+  if (!d2h(k.data(), key, n * 4) || !d2h(meta.data(), d.meta, n * 4) || (imp.loss && !d2h(loss.data(), imp.loss, n * 4)) ||
+      (imp.recv && !d2h(recv.data(), imp.recv, n * 4)) || (imp.delay && !d2h(delay.data(), imp.delay, n)) ||
+      (imp.flags && !d2h(flags.data(), imp.flags, n)))
+    return false;
+  const GsImpairCols h = {imp.loss ? loss.data() : nullptr, imp.recv ? recv.data() : nullptr,
+                          imp.delay ? delay.data() : nullptr, imp.flags ? flags.data() : nullptr};
+  for (uint32_t i = 0; i < n; ++i) {
+    const uint32_t b = gs_health_bin(k[i], meta[i], h, i);
+    if (b < GS_HIST_BINS) out[b]++;
+  }
+  return true;
+}
+
+// (*Serf).Stats() of members [first, first + count) — what `consul info` prints as serf_lan / serf_wan
+// (agent/consul/client.go:417, server.go:1733,1744).  Read-only.
+extern "C" int gsim_agent_stats_read(gsim_pool* p, uint32_t first, uint32_t count, gsim_agent_stats* out) {
+  if (!p || !out || count == 0u) return GSIM_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(p->mu);
+  GS_CONTROLLER_ONLY(p);
+  if (first >= p->g.n || count > p->g.n - first) return fail(p, GSIM_ERR_NOT_FOUND, "unknown member");
+  GsPendingAlive pa;
+  gs_pending_alive(p->g, pa);
+  if (!dev(p)->agent_stats(p->d, p->g, p->d.key[p->now & 1u], pa, first, count, reinterpret_cast<GsAgentStats*>(out)))
+    return fail(p, GSIM_ERR_CUDA, "agent_stats");
+  return GSIM_OK;
+}
+
+// memberlist GetHealthScore() of every running member, counted by score: out[0] unimpaired, out[1] impaired.
+extern "C" int gsim_health_histogram(gsim_pool* p, uint64_t out[2][8]) {
+  if (!p || !out) return GSIM_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(p->mu);
+  GS_CONTROLLER_ONLY(p);
+  const GsImpairCols imp = {p->imp_loss, p->imp_recv, p->imp_delay, p->imp_flags};
+  uint64_t h[GS_HIST_BINS];
+  if (!dev(p)->health_histogram(p->d, p->g, p->d.key[p->now & 1u], imp, h))
+    return fail(p, GSIM_ERR_CUDA, "health_histogram");
+  memcpy(out, h, sizeof(h));
+  return GSIM_OK;
+}
+
 extern "C" int gsim_poll_events(gsim_pool* p, gsim_event* out, size_t cap, size_t* n) {
   if (!p || !n || (!out && cap)) return GSIM_ERR_INVALID;
   std::lock_guard<std::mutex> lk(p->mu);

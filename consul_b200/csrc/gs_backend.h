@@ -10,6 +10,7 @@
 
 #include <vector>
 
+#include "gs_agent.h"
 #include "gs_core.h"
 
 struct GsRecount {
@@ -272,6 +273,16 @@ class GsBackend {
   // kept.  `part` has room for 2 ceil(n_draws / GS_ERR_CHUNK) doubles.
   virtual bool coord_error(const GsDev& d, const GsGlobals* g_dev, const GsGlobals& g, uint32_t now, uint32_t n_draws,
                            uint32_t salt, uint64_t* key, uint32_t* val, double* part, double* out);
+  // ---- per-agent observation (gs_agent.h, DESIGN.md §3.8) ------------------------------------------
+  // Read-only; `key` is the key buffer of the current tick and `out` host memory.  Defined in gs_api.cpp
+  // through the copy primitives every backend has, which is what the host emulation runs; the CUDA backend
+  // replaces each with sm_90a kernels in one submission and one wait.
+  // out[x] = gs_agent_stats_row of member first + x (est[] counted over every member first)
+  virtual bool agent_stats(const GsDev& d, const GsGlobals& g, const uint32_t* key, const GsPendingAlive& pa,
+                           uint32_t first, uint32_t count, GsAgentStats* out);
+  // out[b] = members in bin b of gs_health_bin, over every member
+  virtual bool health_histogram(const GsDev& d, const GsGlobals& g, const uint32_t* key, const GsImpairCols& imp,
+                                uint64_t out[GS_HIST_BINS]);
   // counts over members [first, first + count) (a rank of a sharded pool counts its own rows)
   virtual bool recount(const GsDev& d, const GsGlobals* g_dev, const GsGlobals& g, uint32_t now, uint32_t first,
                        uint32_t count, GsRecount* out) = 0;

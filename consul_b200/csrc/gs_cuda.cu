@@ -1157,6 +1157,56 @@ __global__ void __launch_bounds__(GS_BLOCK)
   if (threadIdx.x < 4 && s[threadIdx.x]) atomicAdd(&out[threadIdx.x], s[threadIdx.x]);
 }
 
+// ---- per-agent observation (gs_agent.h): read-only ----------------------------------------------------
+// gsim_agent_stats_read, first pass over the key column: est[r] += established members of rank r.
+__global__ void __launch_bounds__(GS_BLOCK)
+    gs_agent_est_kernel(const uint32_t* __restrict__ key, uint32_t n, uint32_t* est) {
+  uint32_t c[4] = {0u, 0u, 0u, 0u};
+  for (size_t i = (size_t)blockIdx.x * GS_BLOCK + threadIdx.x; i < n; i += (size_t)gridDim.x * GS_BLOCK) {
+    const uint32_t r1 = gs_established_rank1(key[i]);
+#pragma unroll
+    for (uint32_t r = 0; r < 4u; ++r) c[r] += r1 == r + 1u ? 1u : 0u;
+  }
+#pragma unroll
+  for (uint32_t r = 0; r < 4u; ++r) {
+    const uint32_t s = __reduce_add_sync(0xFFFFFFFFu, c[r]);
+    if ((threadIdx.x & 31u) == 0u && s) atomicAdd(&est[r], s);
+  }
+}
+
+struct GsClassMasks {
+  uint32_t m[3];
+};
+
+// ... second pass: thread x computes the stats of member first + x.
+__global__ void __launch_bounds__(GS_BLOCK)
+    gs_agent_stats_kernel(GsAgentCols c, GsClassMasks cm, const uint32_t* __restrict__ est,
+                          const __grid_constant__ GsPendingAlive pa, uint32_t first, uint32_t count, GsAgentStats* out) {
+  const uint32_t x = blockIdx.x * GS_BLOCK + threadIdx.x;
+  if (x >= count) return;
+  const uint32_t e[4] = {est[0], est[1], est[2], est[3]};
+  out[x] = gs_agent_stats_row(c, cm.m, e, pa, first + x);
+}
+
+// gsim_health_histogram: out[b] += members in bin b, aggregated per warp (one shared atomic per distinct bin
+// of 32 members) and per CTA (one global atomic per bin).
+__global__ void __launch_bounds__(GS_BLOCK)
+    gs_health_hist_kernel(const uint32_t* __restrict__ key, const uint32_t* __restrict__ meta, GsImpairCols imp,
+                          uint32_t n, unsigned long long* out) {
+  __shared__ uint32_t s[GS_HIST_BINS];
+  if (threadIdx.x < GS_HIST_BINS) s[threadIdx.x] = 0u;
+  __syncthreads();
+  const uint32_t lane = threadIdx.x & 31u;
+  for (size_t i0 = (size_t)blockIdx.x * GS_BLOCK; i0 < n; i0 += (size_t)gridDim.x * GS_BLOCK) {
+    const size_t i = i0 + threadIdx.x;
+    const uint32_t b = i < n ? gs_health_bin(key[i], meta[i], imp, (uint32_t)i) : GS_HIST_NONE;
+    const unsigned peers = __match_any_sync(0xFFFFFFFFu, b);
+    if (b != GS_HIST_NONE && lane == (uint32_t)__ffs(peers) - 1u) atomicAdd(&s[b], (uint32_t)__popc(peers));
+  }
+  __syncthreads();
+  if (threadIdx.x < GS_HIST_BINS && s[threadIdx.x]) atomicAdd(&out[threadIdx.x], (unsigned long long)s[threadIdx.x]);
+}
+
 // Tick launches use programmatic stream serialization (PDL) so consecutive ticks overlap
 // launch latency and prologue with the previous tick's tail.
 static cudaError_t gs_launch_tick(uint32_t blocks, cudaStream_t stream, const GsDev& d,
@@ -1978,6 +2028,45 @@ class CudaBackend : public GsBackend {
       ++launches_;
     }
     return ok(cudaGetLastError(), "recount launch") && d2h(out, dr, sizeof(GsRecount));
+  }
+  // ---- per-agent observation: one submission, one wait -------------------------------------------------
+  bool agent_stats(const GsDev& d, const GsGlobals& g, const uint32_t* key, const GsPendingAlive& pa, uint32_t first,
+                   uint32_t count, GsAgentStats* out) override {
+    cudaSetDevice(dev_);
+    uint32_t* est = reinterpret_cast<uint32_t*>(scratch_);
+    if (!ok(cudaMemsetAsync(est, 0, 16, stream_), "memset")) return false;
+    if (!g.graph_n && g.n) {  // a CSR pool's list is the agent's row: no pool-wide counts
+      const uint32_t blocks = (g.n + GS_BLOCK - 1) / GS_BLOCK < sms_ * 8u ? (g.n + GS_BLOCK - 1) / GS_BLOCK : sms_ * 8u;
+      gs_agent_est_kernel<<<blocks, GS_BLOCK, 0, stream_>>>(key, g.n, est);
+      ++launches_;
+    }
+    const size_t bytes = (size_t)count * sizeof(GsAgentStats);
+    GsAgentStats* dout = nullptr;
+    if (!ok(cudaGetLastError(), "agent counts launch") ||
+        !ok(cudaMallocAsync(reinterpret_cast<void**>(&dout), bytes, stream_), "malloc"))
+      return false;
+    const GsAgentCols c = {key, d.meta, d.heard, d.queued, d.ltime_member, d.ltime_event,
+                           g.graph_n ? d.row_ptr : nullptr, g.graph_n ? d.col_idx : nullptr};
+    GsClassMasks cm;
+    memcpy(cm.m, g.class_mask, sizeof(cm.m));
+    gs_agent_stats_kernel<<<(count + GS_BLOCK - 1) / GS_BLOCK, GS_BLOCK, 0, stream_>>>(c, cm, est, pa, first, count, dout);
+    ++launches_;
+    const bool okk = ok(cudaGetLastError(), "agent stats launch") &&
+                     ok(cudaMemcpyAsync(out, dout, bytes, cudaMemcpyDeviceToHost, stream_), "d2h");
+    cudaFreeAsync(dout, stream_);
+    return ok(cudaStreamSynchronize(stream_), "agent stats sync") && okk;
+  }
+  bool health_histogram(const GsDev& d, const GsGlobals& g, const uint32_t* key, const GsImpairCols& imp,
+                        uint64_t out[GS_HIST_BINS]) override {
+    cudaSetDevice(dev_);
+    unsigned long long* h = reinterpret_cast<unsigned long long*>(scratch_);
+    if (!ok(cudaMemsetAsync(h, 0, GS_HIST_BINS * 8, stream_), "memset")) return false;
+    if (g.n) {
+      const uint32_t blocks = (g.n + GS_BLOCK - 1) / GS_BLOCK < sms_ * 8u ? (g.n + GS_BLOCK - 1) / GS_BLOCK : sms_ * 8u;
+      gs_health_hist_kernel<<<blocks, GS_BLOCK, 0, stream_>>>(key, d.meta, imp, g.n, h);
+      ++launches_;
+    }
+    return ok(cudaGetLastError(), "health histogram launch") && d2h(out, h, GS_HIST_BINS * 8);
   }
   bool state_hash(const GsDev& d, const GsGlobals* g_dev, const GsGlobals& g, uint32_t now,
                   uint64_t out[4]) override {

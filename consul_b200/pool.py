@@ -10,8 +10,11 @@ from dataclasses import dataclass
 import numpy as np
 
 from . import _lib
-from ._lib import (COLUMNS, GSIM_MAX_RUMORS, GSIM_MAX_SUSPICION_SLOTS, STAT_NAMES, GsimConfig,
-                   GsimEvent, GsimMember, GsimMemberDesc, GsimRumorInfo, GsimStats)
+from ._lib import (AGENT_STATS_FIELDS, COLUMNS, GSIM_MAX_RUMORS, GSIM_MAX_SUSPICION_SLOTS, STAT_NAMES,
+                   GsimConfig, GsimEvent, GsimMember, GsimMemberDesc, GsimRumorInfo, GsimStats)
+
+# gsim_agent_stats, one uint32 per field
+AGENT_STATS_DTYPE = np.dtype([(n, np.uint32) for n in AGENT_STATS_FIELDS])
 
 IMPAIR_NO_TCP = 1  # GSIM_IMPAIR_NO_TCP
 
@@ -343,6 +346,21 @@ class Pool:
         out = C.c_uint32()
         self._ck(self.lib.gsim_num_nodes(self.h, observer, C.byref(out)))
         return out.value
+
+    def agent_stats(self, first: int = 0, count: int | None = None) -> np.ndarray:
+        """(*Serf).Stats() of members [first, first + count), computed on the device, as a structured array
+        with the fields of AGENT_STATS_DTYPE (DESIGN.md §3.8)."""
+        if count is None:
+            count = self.stats()["n_members"] - first
+        out = np.zeros(max(count, 0), dtype=AGENT_STATS_DTYPE)
+        self._ck(self.lib.gsim_agent_stats_read(self.h, first, count, out.ctypes.data_as(C.c_void_p)))
+        return out
+
+    def health_histogram(self) -> np.ndarray:
+        """Running members by health score (awareness): row 0 without an impairment, row 1 with one."""
+        out = np.zeros((2, 8), dtype=np.uint64)
+        self._ck(self.lib.gsim_health_histogram(self.h, out.ctypes.data_as(C.POINTER(C.c_uint64))))
+        return out
 
     def poll_events(self, cap: int = 65536):
         buf = (GsimEvent * cap)()

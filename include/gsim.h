@@ -429,6 +429,33 @@ int gsim_members(gsim_pool* p, uint32_t observer, gsim_member* out, size_t cap, 
 /* (*Serf).NumNodes() — agent/router/router.go:62-67. */
 int gsim_num_nodes(gsim_pool* p, uint32_t observer, uint32_t* n);
 
+/* Per-agent (*Serf).Stats() — the serf_lan / serf_wan sections of `consul info` (agent/consul/client.go:417,
+ * server.go:1733,1744) — and Lifeguard health scores, computed on the device (DESIGN.md §3.8).  Read-only: pool
+ * state, digest, counters, schedule and event log stay as they were.  Each call is one submission and one wait;
+ * no column is copied to the host.  Sharded pools serve both from rank 0 (GSIM_ERR_STATE elsewhere). */
+typedef struct gsim_agent_stats {
+  /* [U] serf.Stats "members" / "failed" / "left": the agent's member list as gsim_members(observer = agent)
+   * returns it, its entries with status FAILED, and those with status LEFT */
+  uint32_t members, failed, left;
+  uint32_t health_score; /* [U] memberlist.GetHealthScore(): awareness, 0 .. awareness_max_multiplier - 1 */
+  /* [U] serf.Stats "member_time" / "event_time" / "query_time": the agent's Lamport clocks.  Queries are not
+   * simulated, so query_time stays at the 1 gsim_member_add starts every clock at. */
+  uint32_t member_time, event_time, query_time;
+  /* [U] serf.Stats "intent_queue" / "event_queue" / "query_queue": TransmitLimitedQueue.NumQueued of serf's
+   * broadcast queues, the tracked join / leave intents and user events the agent still retransmits;
+   * query_queue is 0 */
+  uint32_t intent_queue, event_queue, query_queue;
+  uint32_t memberlist_queue; /* [U] memberlist TransmitLimitedQueue.NumQueued: alive / update broadcasts */
+  uint32_t running;          /* truth UP: 0 for crashed, paused and gone members */
+} gsim_agent_stats;
+/* out[x] = the stats of member first + x, x < count.  GSIM_ERR_INVALID: count == 0 or out NULL;
+ * GSIM_ERR_NOT_FOUND: first + count > created ids. */
+int gsim_agent_stats_read(gsim_pool* p, uint32_t first, uint32_t count, gsim_agent_stats* out);
+/* Running (truth UP) members counted by health score: out[0][s] those without an impairment, out[1][s] those
+ * with one (any of the four gsim_impair_dir_get values non-zero).  Paused members do not run and are not
+ * counted.  GSIM_ERR_INVALID: out NULL. */
+int gsim_health_histogram(gsim_pool* p, uint64_t out[2][8]);
+
 typedef struct gsim_event {
   uint32_t tick;
   uint32_t type;     /* GSIM_EVENT_* */

@@ -276,11 +276,19 @@ class Serf {
   }
   void RemoveFailedNode(const std::string& node) { force_leave(node, 0); }
   void RemoveFailedNodePrune(const std::string& node) { force_leave(node, 1); }
+  // serf's key set for this agent ([U] serf.Stats), computed on the device, plus the pool's tick.  Nothing is
+  // encrypted inside the simulator and the model never resets a coordinate.
   std::map<std::string, std::string> Stats() {
-    gsim_stats st;
-    p_.check(gsim_stats_get(p_.h_, &st));
-    return {{"members", std::to_string(st.n_members)}, {"failed", std::to_string(st.n_view_dead)},
-            {"left", std::to_string(st.n_view_left)}, {"tick", std::to_string(st.tick)}};
+    gsim_agent_stats a;
+    p_.check(gsim_agent_stats_read(p_.h_, id_, 1, &a));
+    auto u = [](uint32_t v) { return std::to_string(v); };
+    return {{"members", u(a.members)},           {"failed", u(a.failed)},
+            {"left", u(a.left)},                 {"health_score", u(a.health_score)},
+            {"member_time", u(a.member_time)},   {"event_time", u(a.event_time)},
+            {"query_time", u(a.query_time)},     {"intent_queue", u(a.intent_queue)},
+            {"event_queue", u(a.event_queue)},   {"query_queue", u(a.query_queue)},
+            {"encrypted", "false"},              {"coordinate_resets", "0"},
+            {"tick", u(gsim_now(p_.h_))}};
   }
   const Config& config() const { return conf_; }
   uint32_t id() const { return id_; }
