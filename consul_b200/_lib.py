@@ -126,6 +126,11 @@ SIGNATURES = [
     ("gsim_impair_dir_many", _i32, [_P, C.POINTER(_u32), _sz, _u32, _u32, _u32, _u32]),
     ("gsim_impair_dir_fraction", _i32, [_P, _u32, _u32, _u32, _u32, _u32, _u32, C.POINTER(_u32)]),
     ("gsim_impair_dir_get", _i32, [_P, _u32, C.POINTER(_u32), C.POINTER(_u32), C.POINTER(_u32), C.POINTER(_u32)]),
+    ("gsim_impair_flap_many", _i32, [_P, C.POINTER(_u32), _sz, _u32, _u32]),
+    ("gsim_impair_flap_fraction", _i32, [_P, _u32, _u32, _u32, _u32, C.POINTER(_u32)]),
+    ("gsim_impair_flap_get", _i32, [_P, _u32, C.POINTER(_u32), C.POINTER(_u32)]),
+    ("gsim_impair_flap_stats", _i32, [_P, C.POINTER(_u64)]),
+    ("gsim_flap_bad", _i32, [_u64, _u32, _u32, _u32, _u32]),
     ("gsim_pause_many", _i32, [_P, C.POINTER(_u32), _sz, _u32, C.POINTER(_u32)]),
     ("gsim_pause_fraction", _i32, [_P, _u32, _u32, _u32, C.POINTER(_u32)]),
     ("gsim_pause_get", _i32, [_P, _u32, C.POINTER(_u32)]),

@@ -302,6 +302,11 @@ struct gsim_pool {
   // threshold, imp_recv the receive threshold.  Until then the receive threshold is imp_loss itself.
   uint32_t* imp_recv = nullptr;
   uint8_t* imp_flags = nullptr;
+  // ... and intermittent impairment (gsim_impair_flap_*): the schedule column (gs_flap_word per member, 0 =
+  // none), allocated by the first schedule call, and how many members have a schedule.  d.imp_flap points at
+  // the column only while that count and n_impaired are > 0 (a schedule gates an impairment).
+  uint32_t* imp_flap = nullptr;
+  uint32_t n_flap = 0;
   // paused members (gsim_pause_*): the resume-tick column (0 = not paused) and {paused now, resumed Alive,
   // Suspect, Dead}; the first pause allocates the column and pause_cnt_dev, a device copy of the counts that
   // exists only so that snapshots carry them
@@ -1279,11 +1284,14 @@ extern "C" int gsim_join(gsim_pool* p, uint32_t id, const uint32_t* seeds, size_
   uint32_t* ri = row(id);
   if (gs_key_truth(ri[cur]) != GS_TRUTH_UP) return fail(p, GSIM_ERR_STATE, "member is not running");
   // GSIM_IMPAIR_NO_TCP at the joiner or at a seed: the push-pull to that seed cannot connect (only pools
-  // that have the flag column read it)
+  // that have the flag column read it; a member with a flap schedule only while it is in a bad epoch now)
   std::vector<uint8_t> no_tcp(ids.size(), 0u);
   for (size_t x = 0; p->imp_flags && x < ids.size(); ++x) {
     if (!peek(p, p->imp_flags, ids[x], &no_tcp[x])) return fail(p, GSIM_ERR_CUDA, "peek");
     no_tcp[x] &= GSIM_IMPAIR_NO_TCP;
+    uint32_t w = 0u;
+    if (no_tcp[x] && p->d.imp_flap && !peek(p, p->imp_flap, ids[x], &w)) return fail(p, GSIM_ERR_CUDA, "peek");
+    if (w != 0u && !gs_flap_bad(g.seed_lo, g.seed_hi, ids[x], w, p->now)) no_tcp[x] = 0u;
   }
   auto tcp_blocked = [&](uint32_t m) { return no_tcp[std::find(ids.begin(), ids.end(), m) - ids.begin()] != 0u; };
   int okc = 0;
@@ -1704,6 +1712,7 @@ struct HostCoords {
   std::vector<double> coord;
   std::vector<uint32_t> ctag, key;
   std::vector<uint8_t> delay;
+  std::vector<uint32_t> flap;
   GsDev d;
   bool load(GsBackend* be, const GsDev& dd, const GsGlobals& g, uint32_t now, bool keys) {
     const size_t cap = g.cap;
@@ -1718,6 +1727,11 @@ struct HostCoords {
       delay.resize(cap);
       if (!be->d2h(delay.data(), dd.imp_delay, cap)) return false;
       d.imp_delay = delay.data();
+    }
+    if (dd.imp_flap) {
+      flap.resize(cap);
+      if (!be->d2h(flap.data(), dd.imp_flap, cap * 4)) return false;
+      d.imp_flap = flap.data();
     }
     if (keys) {
       key.resize(g.n);
@@ -1740,7 +1754,7 @@ bool GsBackend::coord_rows(const GsDev& d, const GsGlobals& g, uint32_t first, u
   return h2d(rows, out.data(), out.size() * sizeof(GsCoord));
 }
 
-bool GsBackend::coord_pairs(const GsDev& d, const GsGlobals*, const GsGlobals& g, const uint32_t* a, const uint32_t* b,
+bool GsBackend::coord_pairs(const GsDev& d, const GsGlobals*, const GsGlobals& g, uint32_t now, const uint32_t* a, const uint32_t* b,
                             uint32_t n, double* est, double* tru) {
   if (!n) return true;
   HostCoords h;
@@ -1753,7 +1767,7 @@ bool GsBackend::coord_pairs(const GsDev& d, const GsGlobals*, const GsGlobals& g
     gs_coord_pick(h.d.coord, h.d.ctag, g.cap, ha[k], ca);
     gs_coord_pick(h.d.coord, h.d.ctag, g.cap, hb[k], cb);
     he[k] = gs_coord_distance_seconds(ca, cb);
-    ht[k] = gs_model_rtt(g, h.d.imp_delay, ha[k], hb[k]);
+    ht[k] = gs_model_rtt(g, h.d.imp_delay, h.d.imp_flap, ha[k], hb[k], now);
   }
   return h2d(est, he.data(), (size_t)n * 8) && (!tru || h2d(tru, ht.data(), (size_t)n * 8));
 }
@@ -1912,7 +1926,7 @@ extern "C" int gsim_rtt_many(gsim_pool* p, const uint32_t* a, const uint32_t* b,
   double* dt = true_s ? de + n : nullptr;
   std::vector<double> back(true_s ? 2 * n : 0);
   bool okk = dev(p)->h2d_async(da, a, n * 4) && dev(p)->h2d_async(db, b, n * 4) &&
-             dev(p)->coord_pairs(p->d, p->g_dev, p->g, da, db, (uint32_t)n, de, dt);
+             dev(p)->coord_pairs(p->d, p->g_dev, p->g, p->now, da, db, (uint32_t)n, de, dt);
   if (okk && true_s) {
     okk = dev(p)->d2h(back.data(), de, n * 16);
     if (okk) {
@@ -2092,6 +2106,7 @@ static void impair_publish(gsim_pool* p) {
   p->d.imp_delay = p->n_impaired ? p->imp_delay : nullptr;
   p->d.imp_recv = p->n_impaired ? (p->imp_recv ? p->imp_recv : p->imp_loss) : nullptr;
   p->d.imp_flags = p->n_impaired ? p->imp_flags : nullptr;
+  p->d.imp_flap = p->n_impaired && p->n_flap ? p->imp_flap : nullptr;
   mark_dirty(p);
 }
 
@@ -2245,6 +2260,103 @@ extern "C" int gsim_impair_dir_get(gsim_pool* p, uint32_t id, uint32_t* send_los
   if (recv_loss_ppm) *recv_loss_ppm = thr_to_ppm(v.recv);
   if (delay_ticks) *delay_ticks = v.delay;
   if (flags) *flags = v.flags;
+  return GSIM_OK;
+}
+
+// ---- intermittent impairment (DESIGN.md §3.5 "Intermittent impairment") ----------------------------
+extern "C" int gsim_flap_bad(uint64_t seed, uint32_t member, uint32_t period_ticks, uint32_t bad_ppm, uint32_t tick) {
+  if (period_ticks == 0u) return 1;  // no schedule: the impairment is always in force
+  if (period_ticks > GS_FLAP_MAX_PERIOD || bad_ppm > 1000000u) return GSIM_ERR_INVALID;
+  return gs_flap_bad((uint32_t)seed, (uint32_t)(seed >> 32), member, gs_flap_word(period_ticks, bad_ppm), tick) ? 1 : 0;
+}
+
+static int flap_check(gsim_pool* p, uint32_t period_ticks, uint32_t bad_ppm) {
+  if (p->sharded) return fail(p, GSIM_ERR_STATE, "intermittent impairment is not supported on sharded pools");
+  if (period_ticks > GS_FLAP_MAX_PERIOD) return fail(p, GSIM_ERR_INVALID, "period_ticks must be <= 4095");
+  if (bad_ppm > 1000000u) return fail(p, GSIM_ERR_INVALID, "bad_ppm must be <= 1000000");
+  return GSIM_OK;
+}
+
+static bool flap_alloc(gsim_pool* p) {
+  if (p->imp_flap) return true;
+  uint32_t* col = nullptr;
+  if (!alloc_col(p, &col, p->g.cap) || !dev(p)->fill32(col, 0u, p->g.cap)) return false;
+  p->imp_flap = col;
+  return true;
+}
+
+// members with a schedule, counted from the column (after a restore)
+static bool flap_recount(gsim_pool* p) {
+  p->n_flap = 0;
+  if (p->imp_flap && p->g.n) {
+    std::vector<uint32_t> col(p->g.n);
+    if (!dev(p)->d2h(col.data(), p->imp_flap, col.size() * 4)) return false;
+    for (uint32_t w : col) p->n_flap += w != 0u ? 1u : 0u;
+  }
+  impair_publish(p);
+  return true;
+}
+
+static uint32_t flap_word_of(uint32_t period_ticks, uint32_t bad_ppm) {
+  return period_ticks ? gs_flap_word(period_ticks, bad_ppm) : 0u;
+}
+
+extern "C" int gsim_impair_flap_many(gsim_pool* p, const uint32_t* ids, size_t n, uint32_t period_ticks,
+                                     uint32_t bad_ppm) {
+  if (!p || (!ids && n)) return GSIM_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(p->mu);
+  if (int rc = flap_check(p, period_ticks, bad_ppm)) return rc;
+  for (size_t x = 0; x < n; ++x)
+    if (ids[x] >= p->g.n) return fail(p, GSIM_ERR_NOT_FOUND, "unknown member");
+  const uint32_t w = flap_word_of(period_ticks, bad_ppm);
+  if (!p->imp_flap && w == 0u) return GSIM_OK;  // clearing on a pool that never had a schedule
+  if (!flap_alloc(p)) return fail(p, GSIM_ERR_NOMEM, "schedule column");
+  for (size_t x = 0; x < n; ++x) {
+    uint32_t old;
+    if (!peek(p, p->imp_flap, ids[x], &old)) return fail(p, GSIM_ERR_CUDA, "peek");
+    if (!poke(p, p->imp_flap, ids[x], w)) return fail(p, GSIM_ERR_CUDA, "poke");
+    p->n_flap = p->n_flap - (old != 0u ? 1u : 0u) + (w != 0u ? 1u : 0u);
+  }
+  impair_publish(p);
+  return GSIM_OK;
+}
+
+extern "C" int gsim_impair_flap_fraction(gsim_pool* p, uint32_t member_ppm, uint32_t salt, uint32_t period_ticks,
+                                         uint32_t bad_ppm, uint32_t* n_selected) {
+  if (!p || member_ppm > 1000000u) return GSIM_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(p->mu);
+  if (int rc = flap_check(p, period_ticks, bad_ppm)) return rc;
+  const uint32_t w = flap_word_of(period_ticks, bad_ppm);
+  if (!flap_alloc(p)) return fail(p, GSIM_ERR_NOMEM, "schedule column");
+  if (!upload_globals(p)) return fail(p, GSIM_ERR_CUDA, "upload");
+  uint32_t counts[2] = {0, 0};
+  if (!dev(p)->flap_fraction(p->d, p->g_dev, p->g, p->imp_flap, ppm_to_thr(member_ppm), salt, w, counts))
+    return fail(p, GSIM_ERR_CUDA, "flap_fraction");
+  p->n_flap = p->n_flap - counts[1] + (w != 0u ? counts[0] : 0u);
+  if (n_selected) *n_selected = counts[0];
+  impair_publish(p);
+  return GSIM_OK;
+}
+
+extern "C" int gsim_impair_flap_get(gsim_pool* p, uint32_t id, uint32_t* period_ticks, uint32_t* bad_ppm) {
+  if (!p) return GSIM_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(p->mu);
+  if (p->sharded) return fail(p, GSIM_ERR_STATE, "intermittent impairment is not supported on sharded pools");
+  if (id >= p->g.n) return fail(p, GSIM_ERR_NOT_FOUND, "unknown member");
+  uint32_t w = 0u;
+  if (p->imp_flap && !peek(p, p->imp_flap, id, &w)) return fail(p, GSIM_ERR_CUDA, "peek");
+  if (period_ticks) *period_ticks = w >> GS_FLAP_PPM_BITS;
+  if (bad_ppm) *bad_ppm = w & ((1u << GS_FLAP_PPM_BITS) - 1u);
+  return GSIM_OK;
+}
+
+extern "C" int gsim_impair_flap_stats(gsim_pool* p, uint64_t out[2]) {
+  if (!p || !out) return GSIM_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(p->mu);
+  if (p->sharded) return fail(p, GSIM_ERR_STATE, "intermittent impairment is not supported on sharded pools");
+  out[0] = out[1] = 0u;
+  if (!p->imp_flap) return GSIM_OK;
+  if (!dev(p)->flap_stats(p->g, p->imp_flap, p->now, out)) return fail(p, GSIM_ERR_CUDA, "flap_stats");
   return GSIM_OK;
 }
 
@@ -3299,7 +3411,8 @@ struct SnapCol {
   uint32_t planes;   // equally sized, each a multiple of 4 bytes
   bool may_fill;     // planes may be stored as a repeated word
 };
-static std::vector<SnapCol> snap_cols(gsim_pool* p, bool with_impairment, bool with_pause, bool with_reach) {
+static std::vector<SnapCol> snap_cols(gsim_pool* p, bool with_impairment, bool with_pause, bool with_reach,
+                                      bool with_flap) {
   const GsDev& d = p->d;
   const size_t cap = p->g.cap;
   std::vector<SnapCol> v;
@@ -3339,6 +3452,7 @@ static std::vector<SnapCol> snap_cols(gsim_pool* p, bool with_impairment, bool w
     add(p->pause_until, cap * 4);
     add(p->pause_cnt_dev, 4 * 8, 1, false);
   }
+  if (with_flap) add(p->imp_flap, cap * 4);
   add(d.stats, GSIM_STAT_COUNT * 8, 1, false); add(d.heard_cnt, 32 * 4, 1, false); add(d.conv_tick, 32 * 4, 1, false);
   add(d.crashed_alive, 4, 1, false); add(d.crashed_dead_tick, 4, 1, false);
   return v;
@@ -3368,6 +3482,7 @@ static uint32_t snap_layout(const gsim_pool* p) {
   if (p->pause_until) m |= 32u;  // the pause column and statistics (restore allocates them when the pool has none)
   if (p->imp_recv) m |= 64u;     // the reachability columns (with bit 8; restore allocates them when the pool has none)
   if (p->d.pig) m |= 128u;       // owed answers and the piggyback words (GSIM_FLAG_PROBE_PIGGYBACK)
+  if (p->imp_flap) m |= 256u;    // the flap schedule column (restore allocates it when the pool has none)
   return m;
 }
 static uint64_t snap_graph_hash(const gsim_pool* p) {
@@ -3387,7 +3502,8 @@ static uint64_t snap_graph_hash(const gsim_pool* p) {
 static size_t snap_size(gsim_pool* p) {
   size_t s = sizeof(SnapHeader) + p->sched.size() * sizeof(Sched);
   for (uint32_t r = 0; r < GS_MAX_RUMORS; ++r) s += 12 + p->rh[r].name.size() + p->rh[r].payload.size();
-  for (const SnapCol& c : snap_cols(p, p->imp_loss != nullptr, p->pause_until != nullptr, p->imp_recv != nullptr))
+  for (const SnapCol& c : snap_cols(p, p->imp_loss != nullptr, p->pause_until != nullptr, p->imp_recv != nullptr,
+                                    p->imp_flap != nullptr))
     s += c.bytes + 4u * c.planes;  // upper bound: every plane raw
   return s;
 }
@@ -3437,7 +3553,8 @@ extern "C" int gsim_snapshot(gsim_pool* p, void* out, size_t cap_bytes, size_t* 
   }
   if (p->pause_cnt_dev && !dev(p)->h2d(p->pause_cnt_dev, p->pause_cnt, sizeof(p->pause_cnt)))
     return fail(p, GSIM_ERR_CUDA, "h2d");
-  for (const SnapCol& c : snap_cols(p, p->imp_loss != nullptr, p->pause_until != nullptr, p->imp_recv != nullptr)) {
+  for (const SnapCol& c : snap_cols(p, p->imp_loss != nullptr, p->pause_until != nullptr, p->imp_recv != nullptr,
+                                    p->imp_flap != nullptr)) {
     const size_t pb = c.bytes / c.planes;
     for (uint32_t q = 0; q < c.planes; ++q) {
       uint8_t* raw = w + 4;
@@ -3467,7 +3584,7 @@ extern "C" int gsim_restore(gsim_pool* p, const void* blob, size_t n_bytes) {
   // geometry and peer graph must be this pool's before a single plane is copied.
   if (h.cap != p->g.cap || h.g.cap != p->g.cap || h.g.n > p->cfg.capacity || h.g.n > p->g.cap ||
       h.g.ring_mask != p->g.ring_mask || (h.g.pp_interval != 0u) != (p->g.pp_interval != 0u) ||
-      (h.layout & ~104u) != (snap_layout(p) & ~104u) || (h.layout & 72u) == 64u || h.g.world != p->g.world || h.g.key_stride != p->g.key_stride ||
+      (h.layout & ~360u) != (snap_layout(p) & ~360u) || (h.layout & 72u) == 64u || h.g.world != p->g.world || h.g.key_stride != p->g.key_stride ||
       h.g.rows_per_rank != p->g.rows_per_rank || h.g.phase_group != p->g.phase_group ||
       h.g.graph_n != p->g.graph_n || h.graph_hash != snap_graph_hash(p) || h.n_established > h.g.n)
     return fail(p, GSIM_ERR_INVALID, "snapshot does not match this pool (capacity, column set, sharding or peer graph)");
@@ -3493,7 +3610,9 @@ extern "C" int gsim_restore(gsim_pool* p, const void* blob, size_t n_bytes) {
   if (blob_reach && !reach_alloc(p)) return fail(p, GSIM_ERR_NOMEM, "reachability columns");
   const bool blob_paused = (h.layout & 32u) != 0u;
   if (blob_paused && !pause_alloc(p)) return fail(p, GSIM_ERR_NOMEM, "pause column");
-  for (const SnapCol& c : snap_cols(p, blob_impaired, blob_paused, blob_reach)) {
+  const bool blob_flap = (h.layout & 256u) != 0u;
+  if (blob_flap && !flap_alloc(p)) return fail(p, GSIM_ERR_NOMEM, "schedule column");
+  for (const SnapCol& c : snap_cols(p, blob_impaired, blob_paused, blob_reach, blob_flap)) {
     if (c.may_fill) {  // plane by plane: a device fill or a copy
       const size_t pb = c.bytes / c.planes;
       for (uint32_t q = 0; q < c.planes; ++q) {
@@ -3538,6 +3657,8 @@ extern "C" int gsim_restore(gsim_pool* p, const void* blob, size_t n_bytes) {
     return fail(p, GSIM_ERR_CUDA, "fill");
   // ... and one without the pause column a pool nobody in it is paused
   if (!blob_paused && p->pause_until && !dev(p)->fill32(p->pause_until, 0u, p->g.cap)) return fail(p, GSIM_ERR_CUDA, "fill");
+  // ... and one without the schedule column a pool in which nobody has a schedule
+  if (!blob_flap && p->imp_flap && !dev(p)->fill32(p->imp_flap, 0u, p->g.cap)) return fail(p, GSIM_ERR_CUDA, "fill");
   if (!dev(p)->sync()) return fail(p, GSIM_ERR_CUDA, "sync");  // every plane has left the caller's blob
   // ... and one without the reachability columns a pool whose settings are all symmetric
   if (!blob_reach && p->imp_recv) {
@@ -3563,7 +3684,7 @@ extern "C" int gsim_restore(gsim_pool* p, const void* blob, size_t n_bytes) {
   p->n_established = h.n_established;
   p->g_dirty = true;
   counts_invalidate(p);
-  if (!impair_recount(p)) return fail(p, GSIM_ERR_CUDA, "d2h");
+  if (!impair_recount(p) || !flap_recount(p)) return fail(p, GSIM_ERR_CUDA, "d2h");
   if (!poke(p, p->d.tick_base, 0, p->now) || !reset_tick_flags(p) || !reset_qstate(p)) return fail(p, GSIM_ERR_CUDA, "poke");
   uint32_t zero2[2] = {0, 0};
   if (!dev(p)->h2d(p->d.evlog_cursor, zero2, 8)) return fail(p, GSIM_ERR_CUDA, "h2d");

@@ -236,6 +236,36 @@ class GsBackend {
     const GsImpairVal v = {loss, loss, delay, 0u};
     return impair_dir_fraction(d, g_dev, g, c, thr, salt, v, counts);
   }
+  // Intermittent impairment (gs_core.h; col is the caller's schedule column).  flap_fraction: gs_flap_row(w)
+  // over every member, counts as for impair_dir_fraction; flap_stats: out[0] = members with a schedule, out[1]
+  // = those of them in a bad epoch at tick now.  Defined here through the copy primitives every backend has,
+  // which is what the host emulation runs; the CUDA backend replaces them with gs_flap_kernel and
+  // gs_flap_stats_kernel.
+  virtual bool flap_fraction(const GsDev& d, const GsGlobals* /*g_dev*/, const GsGlobals& g, uint32_t* col,
+                             uint32_t thr, uint32_t salt, uint32_t w, uint32_t counts[2]) {
+    counts[0] = counts[1] = 0u;
+    if (!g.n) return true;
+    std::vector<uint32_t> key(g.n), fc(g.n);
+    if (!d2h(key.data(), d.key[0], (size_t)g.n * 4) || !d2h(fc.data(), col, (size_t)g.n * 4)) return false;
+    for (uint32_t i = 0; i < g.n; ++i) {
+      const uint32_t r = gs_flap_row(key[i], fc.data(), g.seed_lo, g.seed_hi, i, thr, salt, w);
+      counts[0] += r & 1u;
+      counts[1] += (r >> 1) & 1u;
+    }
+    return h2d(col, fc.data(), (size_t)g.n * 4);
+  }
+  virtual bool flap_stats(const GsGlobals& g, const uint32_t* col, uint32_t now, uint64_t out[2]) {
+    out[0] = out[1] = 0u;
+    if (!g.n) return true;
+    std::vector<uint32_t> fc(g.n);
+    if (!d2h(fc.data(), col, (size_t)g.n * 4)) return false;
+    for (uint32_t i = 0; i < g.n; ++i) {
+      if (fc[i] == 0u) continue;
+      out[0]++;
+      out[1] += gs_flap_bad(g.seed_lo, g.seed_hi, i, fc[i], now) ? 1u : 0u;
+    }
+    return true;
+  }
   // Paused members (gs_aux.h; pause_until is the caller's column).  pause_rows: gs_pause_row(until) over the
   // `n` distinct members ids[] when ids != nullptr, otherwise over every member whose gs_pause_pick(thr, salt)
   // draw selects it; *n_paused = members paused.  resume_rows: gs_resume_row(t, resume) over every member,
@@ -254,8 +284,8 @@ class GsBackend {
   // host emulation runs; the CUDA backend replaces each with sm_90a kernels.
   // rows[11 x ..] = the published coordinate (gs_coord_pick) of member first + x
   virtual bool coord_rows(const GsDev& d, const GsGlobals& g, uint32_t first, uint32_t count, double* rows);
-  // est[k] = the distance between a[k] and b[k]; tru[k] (tru may be null) = gs_model_rtt(a[k], b[k])
-  virtual bool coord_pairs(const GsDev& d, const GsGlobals* g_dev, const GsGlobals& g, const uint32_t* a,
+  // est[k] = the distance between a[k] and b[k]; tru[k] (tru may be null) = gs_model_rtt(a[k], b[k]) at tick now
+  virtual bool coord_pairs(const GsDev& d, const GsGlobals* g_dev, const GsGlobals& g, uint32_t now, const uint32_t* a,
                            const uint32_t* b, uint32_t n, double* est, double* tru);
   // key[x] = gs_dist_key of the distance from `from` to ids[x] (ids null: to member x), val[x] = that id; or
   // (router) gs_router_entry at tick now.  ids may be val.

@@ -64,7 +64,9 @@ enum {
   GS_PUR_PUSHPULL = 7,
   // 8 = GS_PUR_COORD (gs_coord.h)
   GS_PUR_IMPAIR = 9,
-  GS_PUR_PAUSE = 10
+  GS_PUR_PAUSE = 10,
+  // 11 = gsim_coordinate_error's sample draws (GS_PUR_COORD_SAMPLE)
+  GS_PUR_FLAP = 12
 };
 // Loss "kind" (folded into the counter) — one draw per simulated UDP packet.
 enum {
@@ -318,6 +320,39 @@ GS_HD uint32_t gs_impair_row(uint32_t key, const GsImpairCols& c, uint32_t seed_
   return was ? 3u : 1u;
 }
 
+// Intermittent impairment (gsim_impair_flap_*): a member's schedule word is period << 20 | bad_ppm, 0 for
+// none.  Time is cut into epochs of `period` ticks, shifted per member by a phase drawn once; each epoch is
+// bad with probability bad_ppm / 1e6, and the member's impairment is in force only during bad epochs.
+#define GS_FLAP_PPM_BITS 20u
+#define GS_FLAP_MAX_PERIOD 4095u
+GS_HD uint32_t gs_flap_word(uint32_t period, uint32_t bad_ppm) { return period << GS_FLAP_PPM_BITS | bad_ppm; }
+
+// Is member m in a bad epoch at tick t under schedule word w (w != 0)?  phase = philox(m, ~0, FLAP).y mod
+// period; epoch = (t + phase) / period in 64 bits; bad iff philox(m, epoch, FLAP).x < thr(bad_ppm), the ppm
+// threshold floor(ppm 2^32 / 1e6), except that 1e6 is bad in every epoch.
+GS_HD bool gs_flap_bad(uint32_t seed_lo, uint32_t seed_hi, uint32_t m, uint32_t w, uint32_t t) {
+  const uint32_t period = w >> GS_FLAP_PPM_BITS, ppm = w & ((1u << GS_FLAP_PPM_BITS) - 1u);
+  if (ppm >= 1000000u) return true;
+  if (ppm == 0u) return false;
+  const uint32_t phase = gs_philox(seed_lo, seed_hi, m, 0xFFFFFFFFu, GS_PUR_FLAP, 0u).y % period;
+  // (t + phase) / period without a 64-bit division: t = q period + r, and r + phase < 2 period
+  const uint32_t q = t / period, r = t - q * period;
+  const uint32_t epoch = q + (r + phase >= period ? 1u : 0u);
+  const uint32_t thr = (uint32_t)(((uint64_t)ppm << 32) / 1000000u);
+  return gs_philox(seed_lo, seed_hi, m, epoch, GS_PUR_FLAP, 0u).x < thr;
+}
+
+// gsim_impair_flap_fraction for member i: the selection of gs_impair_row (same draw, so a salt picks the
+// same members), writing schedule word w.  Returns bit 0 = selected, bit 1 = it had a schedule before.
+GS_HD uint32_t gs_flap_row(uint32_t key, uint32_t* col, uint32_t seed_lo, uint32_t seed_hi, uint32_t i, uint32_t thr,
+                           uint32_t salt, uint32_t w) {
+  if ((key & 3u) != GS_TRUTH_UP) return 0u;
+  if (gs_philox(seed_lo, seed_hi, i, salt, GS_PUR_IMPAIR, 0u).x >= thr) return 0u;
+  const bool was = col[i] != 0u;
+  col[i] = w;
+  return was ? 3u : 1u;
+}
+
 // Retransmit counter of rumor r at member i.  Two rumors share one 16-bit element so that the
 // narrowest column has 2-byte elements: a sharded pool maps every (column, rank) slice with the
 // 2 MB granularity of the virtual-memory API, which then allows 1 Mi members per GPU (1-byte
@@ -478,6 +513,10 @@ struct GsDev {
   // the GS_PIGK smallest by an atomicMin chain; and the pool-wide words
   uint32_t* pig_req;
   GsPig* pig;
+  // intermittent impairment (gsim_impair_flap_*): schedule words (gs_flap_bad), null while no member has a
+  // schedule or nobody is impaired.  Only the impaired row step reads it; last in the struct, so every other
+  // field keeps its offset.
+  const uint32_t* imp_flap;
 };
 
 // Broadcasts piggybacked on probe traffic (GSIM_FLAG_PROBE_PIGGYBACK, DESIGN.md §3.7).

@@ -39,8 +39,10 @@
 namespace {
 
 // COORDS selects the tick-kernel instantiation that carries the network-coordinate update
-// (gs_coord.h, ~150 double-precision operations per direct ack).  The default instantiation
-// contains none of that code, so pools without GSIM_FLAG_COORDINATES pay nothing for it.
+// (gs_coord.h, ~150 double-precision operations per direct ack) and the row step of pools with flap
+// schedules (gsim_impair_flap_*: Philox draws at the register limit).  The default instantiation
+// contains none of that code, so pools with neither pay nothing for it; a pool with schedules runs the
+// COORDS instantiation whether or not it has coordinates (the update is skipped without them).
 template <bool COORDS>
 struct DevSinkT {
   static constexpr bool kCoords = COORDS;
@@ -197,11 +199,27 @@ __device__ __noinline__ void gs_row_step_call(const GsDev* dp, const GsGlobals* 
   gs_row_step_body<false>(*dp, *gp, i, t, t % gp->GI, inb, sink);
 }
 
-// Every generic row step of the tick and window kernels: piggybacking pools call their own step from here, not
-// from inside gs_row_step_call, so that its frame does not stack on top of the default step's.
+// Pools whose impaired members have flap schedules (GsDev::imp_flap set, only with imp_loss) likewise; only
+// the COORDS kernels call it (gs_kernel_extras).
+template <bool COORDS, bool PIG>
+__device__ __noinline__ void gs_row_step_flap_call(const GsDev* dp, const GsGlobals* gp, uint32_t i, uint32_t t,
+                                                   uint32_t inb, uint32_t* s_stat, uint32_t* s_heard, uint32_t* s_q) {
+  DevSinkT<COORDS> sink{s_stat, s_heard, s_q};
+  gs_row_step_body<true, PIG, true>(*dp, *gp, i, t, t % gp->GI, inb, sink);
+}
+
+// Every generic row step of the tick and window kernels: piggybacking and flapping pools call their own step from
+// here, not from inside gs_row_step_call, so that its frame does not stack on top of the default step's.
 template <bool COORDS>
 __device__ __forceinline__ void gs_row_step_any(const GsDev* dp, const GsGlobals* gp, uint32_t i, uint32_t t,
                                                 uint32_t inb, uint32_t* s_stat, uint32_t* s_heard, uint32_t* s_q) {
+  if constexpr (COORDS) {
+    if (dp->imp_flap != nullptr) {
+      if (dp->pig == nullptr) gs_row_step_flap_call<COORDS, false>(dp, gp, i, t, inb, s_stat, s_heard, s_q);
+      else gs_row_step_flap_call<COORDS, true>(dp, gp, i, t, inb, s_stat, s_heard, s_q);
+      return;
+    }
+  }
   if (dp->pig == nullptr) gs_row_step_call<COORDS>(dp, gp, i, t, inb, s_stat, s_heard, s_q);
   else if (dp->imp_loss != nullptr) gs_row_step_pig_call<COORDS, true>(dp, gp, i, t, inb, s_stat, s_heard, s_q);
   else gs_row_step_pig_call<COORDS, false>(dp, gp, i, t, inb, s_stat, s_heard, s_q);
@@ -1047,6 +1065,43 @@ __global__ void __launch_bounds__(GS_BLOCK)
   }
 }
 
+// gsim_impair_flap_fraction: gs_flap_row for member i, counts[0] += selected, counts[1] += selected members
+// that had a schedule before.
+__global__ void __launch_bounds__(GS_BLOCK)
+    gs_flap_kernel(GsDev d, const GsGlobals* __restrict__ gp, uint32_t* col, uint32_t thr, uint32_t salt, uint32_t w,
+                   uint32_t* counts) {
+  const uint32_t i = blockIdx.x * GS_BLOCK + threadIdx.x;
+  uint32_t r = 0u;
+  if (i < gp->n) r = gs_flap_row(d.key[0][i], col, gp->seed_lo, gp->seed_hi, i, thr, salt, w);
+  const unsigned sel = __ballot_sync(0xFFFFFFFFu, r & 1u), was = __ballot_sync(0xFFFFFFFFu, r & 2u);
+  if ((threadIdx.x & 31u) == 0u && sel) {
+    atomicAdd(&counts[0], (uint32_t)__popc(sel));
+    if (was) atomicAdd(&counts[1], (uint32_t)__popc(was));
+  }
+}
+
+// gsim_impair_flap_stats: out[0] += members with a schedule, out[1] += those in a bad epoch at tick now,
+// aggregated per warp (a ballot) and per CTA (one global atomic per count).
+__global__ void __launch_bounds__(GS_BLOCK)
+    gs_flap_stats_kernel(const uint32_t* __restrict__ col, uint32_t n, uint32_t seed_lo, uint32_t seed_hi, uint32_t now,
+                         unsigned long long* out) {
+  __shared__ uint32_t s[2];
+  if (threadIdx.x < 2u) s[threadIdx.x] = 0u;
+  __syncthreads();
+  for (size_t i0 = (size_t)blockIdx.x * GS_BLOCK; i0 < n; i0 += (size_t)gridDim.x * GS_BLOCK) {
+    const size_t i = i0 + threadIdx.x;
+    const uint32_t w = i < n ? col[i] : 0u;
+    const bool bad = w != 0u && gs_flap_bad(seed_lo, seed_hi, (uint32_t)i, w, now);
+    const unsigned has = __ballot_sync(0xFFFFFFFFu, w != 0u), b = __ballot_sync(0xFFFFFFFFu, bad);
+    if ((threadIdx.x & 31u) == 0u && has) {
+      atomicAdd(&s[0], (uint32_t)__popc(has));
+      if (b) atomicAdd(&s[1], (uint32_t)__popc(b));
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x < 2u && s[threadIdx.x]) atomicAdd(&out[threadIdx.x], (unsigned long long)s[threadIdx.x]);
+}
+
 // gsim_pause_many (ids != nullptr: thread x takes member ids[x], no id twice) and gsim_pause_fraction (thread i
 // takes member i): gs_pause_row, *n_paused += members paused.
 __global__ void __launch_bounds__(GS_BLOCK)
@@ -1207,6 +1262,9 @@ __global__ void __launch_bounds__(GS_BLOCK)
   if (threadIdx.x < GS_HIST_BINS && s[threadIdx.x]) atomicAdd(&out[threadIdx.x], (unsigned long long)s[threadIdx.x]);
 }
 
+// The tick and window kernels with COORDS = true: pools with network coordinates or flap schedules.
+static bool gs_kernel_extras(const GsDev& d) { return d.coord != nullptr || d.imp_flap != nullptr; }
+
 // Tick launches use programmatic stream serialization (PDL) so consecutive ticks overlap
 // launch latency and prologue with the previous tick's tail.
 static cudaError_t gs_launch_tick(uint32_t blocks, cudaStream_t stream, const GsDev& d,
@@ -1222,7 +1280,7 @@ static cudaError_t gs_launch_tick(uint32_t blocks, cudaStream_t stream, const Gs
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = pdl ? 1 : 0;
-  return d.coord ? cudaLaunchKernelEx(&cfg, gs_tick_kernel<true>, d, g_dev, k, stretch)
+  return gs_kernel_extras(d) ? cudaLaunchKernelEx(&cfg, gs_tick_kernel<true>, d, g_dev, k, stretch)
                  : cudaLaunchKernelEx(&cfg, gs_tick_kernel<false>, d, g_dev, k, stretch);
 }
 
@@ -1239,9 +1297,9 @@ static cudaError_t gs_launch_window(uint32_t blocks, cudaStream_t stream, const 
   cfg.attrs = attr;
   cfg.numAttrs = pdl ? 1 : 0;
   if (mode & 1u)  // pristine pool: the closed-form instantiation
-    return d.coord ? cudaLaunchKernelEx(&cfg, gs_window_kernel<true, true>, d, g_dev, k_off, n_ticks, mode)
+    return gs_kernel_extras(d) ? cudaLaunchKernelEx(&cfg, gs_window_kernel<true, true>, d, g_dev, k_off, n_ticks, mode)
                    : cudaLaunchKernelEx(&cfg, gs_window_kernel<false, true>, d, g_dev, k_off, n_ticks, mode);
-  return d.coord ? cudaLaunchKernelEx(&cfg, gs_window_kernel<true, false>, d, g_dev, k_off, n_ticks, mode)
+  return gs_kernel_extras(d) ? cudaLaunchKernelEx(&cfg, gs_window_kernel<true, false>, d, g_dev, k_off, n_ticks, mode)
                  : cudaLaunchKernelEx(&cfg, gs_window_kernel<false, false>, d, g_dev, k_off, n_ticks, mode);
 }
 
@@ -1301,8 +1359,8 @@ __global__ void __launch_bounds__(GS_BLOCK)
 }
 
 __global__ void __launch_bounds__(GS_BLOCK)
-    gs_coord_pairs_kernel(GsDev d, const GsGlobals* __restrict__ gp, const uint32_t* a, const uint32_t* b, uint32_t n,
-                          double* est, double* tru) {
+    gs_coord_pairs_kernel(GsDev d, const GsGlobals* __restrict__ gp, uint32_t now, const uint32_t* a, const uint32_t* b,
+                          uint32_t n, double* est, double* tru) {
   const uint32_t k = blockIdx.x * GS_BLOCK + threadIdx.x;
   if (k >= n) return;
   const GsGlobals& g = *gp;
@@ -1311,7 +1369,7 @@ __global__ void __launch_bounds__(GS_BLOCK)
   gs_coord_pick(d.coord, d.ctag, g.cap, i, ci);
   gs_coord_pick(d.coord, d.ctag, g.cap, j, cj);
   est[k] = gs_coord_distance_seconds(ci, cj);
-  if (tru != nullptr) tru[k] = gs_model_rtt(g, d.imp_delay, i, j);
+  if (tru != nullptr) tru[k] = gs_model_rtt(g, d.imp_delay, d.imp_flap, i, j, now);
 }
 
 __global__ void __launch_bounds__(GS_BLOCK)
@@ -1901,6 +1959,28 @@ class CudaBackend : public GsBackend {
     }
     return ok(cudaGetLastError(), "impair launch") && d2h(counts, cnt, 8);
   }
+  bool flap_fraction(const GsDev& d, const GsGlobals* g_dev, const GsGlobals& g, uint32_t* col, uint32_t thr,
+                     uint32_t salt, uint32_t w, uint32_t counts[2]) override {
+    cudaSetDevice(dev_);
+    uint32_t* cnt = reinterpret_cast<uint32_t*>(scratch_);
+    if (!ok(cudaMemsetAsync(cnt, 0, 8, stream_), "memset")) return false;
+    if (g.n) {
+      gs_flap_kernel<<<(g.n + GS_BLOCK - 1) / GS_BLOCK, GS_BLOCK, 0, stream_>>>(d, g_dev, col, thr, salt, w, cnt);
+      ++launches_;
+    }
+    return ok(cudaGetLastError(), "flap launch") && d2h(counts, cnt, 8);
+  }
+  bool flap_stats(const GsGlobals& g, const uint32_t* col, uint32_t now, uint64_t out[2]) override {
+    cudaSetDevice(dev_);
+    unsigned long long* h = reinterpret_cast<unsigned long long*>(scratch_);
+    if (!ok(cudaMemsetAsync(h, 0, 16, stream_), "memset")) return false;
+    if (g.n) {
+      const uint32_t blocks = (g.n + GS_BLOCK - 1) / GS_BLOCK < sms_ * 8u ? (g.n + GS_BLOCK - 1) / GS_BLOCK : sms_ * 8u;
+      gs_flap_stats_kernel<<<blocks, GS_BLOCK, 0, stream_>>>(col, g.n, g.seed_lo, g.seed_hi, now, h);
+      ++launches_;
+    }
+    return ok(cudaGetLastError(), "flap stats launch") && d2h(out, h, 16);
+  }
   bool pause_rows(const GsDev& d, const GsGlobals* g_dev, const GsGlobals& g, uint32_t* pause_until,
                   const uint32_t* ids, uint32_t n, uint32_t thr, uint32_t salt, uint32_t until,
                   uint32_t* n_paused) override {
@@ -1945,11 +2025,11 @@ class CudaBackend : public GsBackend {
     ++launches_;
     return ok(cudaGetLastError(), "coordinate rows launch");
   }
-  bool coord_pairs(const GsDev& d, const GsGlobals* g_dev, const GsGlobals&, const uint32_t* a, const uint32_t* b,
-                   uint32_t n, double* est, double* tru) override {
+  bool coord_pairs(const GsDev& d, const GsGlobals* g_dev, const GsGlobals&, uint32_t now, const uint32_t* a,
+                   const uint32_t* b, uint32_t n, double* est, double* tru) override {
     cudaSetDevice(dev_);
     if (!n) return true;
-    gs_coord_pairs_kernel<<<(n + GS_BLOCK - 1) / GS_BLOCK, GS_BLOCK, 0, stream_>>>(d, g_dev, a, b, n, est, tru);
+    gs_coord_pairs_kernel<<<(n + GS_BLOCK - 1) / GS_BLOCK, GS_BLOCK, 0, stream_>>>(d, g_dev, now, a, b, n, est, tru);
     ++launches_;
     return ok(cudaGetLastError(), "coordinate pairs launch");
   }

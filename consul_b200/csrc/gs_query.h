@@ -21,10 +21,14 @@ GS_DEV void gs_coord_pick(const double* coord, const uint32_t* ctag, size_t cap,
   c.height = base[(size_t)10 * cap];
 }
 
-// The round trip a direct probe between a and b would sample now (gs_coord_on_ack): the latency matrix and
-// the receivers' delays there and back.  `delay` = GsDev::imp_delay (null while nobody is impaired).
-GS_DEV double gs_model_rtt(const GsGlobals& g, const uint8_t* delay, uint32_t a, uint32_t b) {
-  return g.coord_base_rtt_s + (double)(gs_extra(g, delay, a, b) + gs_extra(g, delay, b, a)) * g.tick_seconds;
+// The round trip a direct probe between a and b would sample at tick `now` (gs_coord_on_ack): the latency
+// matrix and the receivers' delays there and back.  `delay` = GsDev::imp_delay (null while nobody is
+// impaired), `flap` = GsDev::imp_flap (a scheduled receiver's delay counts only in its bad epochs).
+GS_DEV double gs_model_rtt(const GsGlobals& g, const uint8_t* delay, const uint32_t* flap, uint32_t a, uint32_t b,
+                           uint32_t now) {
+  return g.coord_base_rtt_s + (double)(gs_extra(g, delay, a, b, gs_imp_on(g, flap, b, now)) +
+                                       gs_extra(g, delay, b, a, gs_imp_on(g, flap, a, now))) *
+                                  g.tick_seconds;
 }
 
 // Sort key of a distance: its IEEE bits.  gs_coord_distance_seconds never returns a negative value, -0 or
@@ -76,7 +80,7 @@ GS_DEV double gs_error_draw(const GsDev& d, const GsGlobals& g, uint32_t now, ui
   GsCoord a, b;
   gs_coord_pick(d.coord, d.ctag, g.cap, i, a);
   gs_coord_pick(d.coord, d.ctag, g.cap, j, b);
-  const double est = gs_coord_distance_seconds(a, b), tru = gs_model_rtt(g, d.imp_delay, i, j);
+  const double est = gs_coord_distance_seconds(a, b), tru = gs_model_rtt(g, d.imp_delay, d.imp_flap, i, j, now);
   return fabs(est - tru) / tru;
 }
 

@@ -201,13 +201,24 @@ GS_DEV GsHot gs_hot(const GsGlobals& g) {
   return h;
 }
 
-// `delay` = the receive-delay column of a pool with impaired members (GsDev::imp_delay), else null:
-// a degraded receiver handles everything delay[dst] ticks late.  The probe fast paths pass null,
-// they only run while nobody is impaired.
+// Is member m's impairment in force at tick t (1) or not (0)?  `flap` = GsDev::imp_flap (schedule words, null
+// while no member has one): a member without a schedule is always impaired, one with a schedule only in its
+// bad epochs (gs_flap_bad).  The row step asks once per member it deals with and hands the answers to the
+// helpers below as `on` bits: bit 0 for the packet's sender (or member i), bit 1 for its receiver (or j).
 template <class G>
-GS_DEV uint32_t gs_extra(const G& g, const uint8_t* delay, uint32_t src, uint32_t dst) {
+GS_DEV uint32_t gs_imp_on(const G& g, const uint32_t* flap, uint32_t m, uint32_t t) {
+  if (flap == nullptr) return 1u;
+  const uint32_t w = flap[m];
+  return w == 0u || gs_flap_bad(g.seed_lo, g.seed_hi, m, w, t) ? 1u : 0u;
+}
+
+// `delay` = the receive-delay column of a pool with impaired members (GsDev::imp_delay), else null:
+// a degraded receiver handles everything delay[dst] ticks late (while its impairment is in force,
+// dst_on).  The probe fast paths pass null, they only run while nobody is impaired.
+template <class G>
+GS_DEV uint32_t gs_extra(const G& g, const uint8_t* delay, uint32_t src, uint32_t dst, uint32_t dst_on = 1u) {
   uint32_t e = g.n_dcs == 0u ? 0u : g.lat[((src / GS_TILE) % g.n_dcs) * GS_MAX_DCS + (dst / GS_TILE) % g.n_dcs];
-  if (delay != nullptr) e += delay[dst];
+  if (delay != nullptr && dst_on != 0u) e += delay[dst];
   return e;
 }
 
@@ -220,35 +231,39 @@ struct GsLossCols {
 };
 
 // The loss rule of one simulated UDP packet from src to dst, on Philox block r of its counter: the
-// pool-wide draw (r.x), then the sender's send threshold (r.y) and the receiver's receive threshold (r.z).
-GS_DEV bool gs_loss_rule(const GsGlobals& g, const GsLossCols& loss, const GsU4& r, uint32_t src, uint32_t dst) {
-  return r.x < g.loss_thr || (loss.send != nullptr && (r.y < loss.send[src] || r.z < loss.recv[dst]));
+// pool-wide draw (r.x), then the sender's send threshold (r.y) and the receiver's receive threshold (r.z),
+// each while that member's impairment is in force (`on` bits 0 and 1, gs_imp_on).
+GS_DEV bool gs_loss_rule(const GsGlobals& g, const GsLossCols& loss, const GsU4& r, uint32_t src, uint32_t dst,
+                         uint32_t on) {
+  return r.x < g.loss_thr ||
+         (loss.send != nullptr && ((r.y < loss.send[src] && (on & 1u)) || (r.z < loss.recv[dst] && (on & 2u))));
 }
 
 // Same draw as gs_lost without touching the counters: re-evaluates, at the ProbeTimeout stage,
 // whether the direct ping/ack of the probe started at t0 were lost (late acks, latency pools).
 GS_DEV bool gs_lost_quiet(const GsGlobals& g, const GsLossCols& loss, uint32_t src, uint32_t dst, uint32_t t,
-                          uint32_t kind, uint32_t idx) {
+                          uint32_t kind, uint32_t idx, uint32_t on = 3u) {
   if (g.loss_thr == 0u && loss.send == nullptr) return false;
   GsU4 r = gs_philox(g.seed_lo, g.seed_hi, src, dst, t, GS_PUR_LOSS | (kind << 8) | (idx << 16));
-  return gs_loss_rule(g, loss, r, src, dst);
+  return gs_loss_rule(g, loss, r, src, dst, on);
 }
 
 // One simulated UDP packet is lost iff its Philox draw says so (gs_loss_rule); counted once.
 template <class Sink>
 GS_DEV bool gs_lost(const GsGlobals& g, const GsLossCols& loss, Sink& sink, uint32_t src, uint32_t dst, uint32_t t,
-                    uint32_t kind, uint32_t idx) {
+                    uint32_t kind, uint32_t idx, uint32_t on = 3u) {
   if (g.loss_thr == 0u && loss.send == nullptr) return false;
   GsU4 r = gs_philox(g.seed_lo, g.seed_hi, src, dst, t, GS_PUR_LOSS | (kind << 8) | (idx << 16));
-  bool lost = gs_loss_rule(g, loss, r, src, dst);
+  bool lost = gs_loss_rule(g, loss, r, src, dst, on);
   if (lost) sink.stat(GS_ST_PACKETS_LOST, 1);
   return lost;
 }
 
-// Does a TCP exchange between members i and j fail (GSIM_IMPAIR_NO_TCP at either end)?  `flags` =
-// GsDev::imp_flags, null unless some member has a directional setting.
-GS_DEV bool gs_no_tcp(const uint8_t* flags, uint32_t i, uint32_t j) {
-  return flags != nullptr && ((flags[i] | flags[j]) & GS_IMPAIR_NO_TCP) != 0u;
+// Does a TCP exchange between members i and j fail (GSIM_IMPAIR_NO_TCP at either end, while in force: `on`
+// bits 0 and 1)?  `flags` = GsDev::imp_flags, null unless some member has a directional setting.
+GS_DEV bool gs_no_tcp(const uint8_t* flags, uint32_t i, uint32_t j, uint32_t on = 3u) {
+  return flags != nullptr && (((flags[i] & GS_IMPAIR_NO_TCP) != 0u && (on & 1u)) ||
+                              ((flags[j] & GS_IMPAIR_NO_TCP) != 0u && (on & 2u)));
 }
 
 // Does member i know member c exists?  Established members are known to everyone; a
@@ -311,7 +326,7 @@ __device__ __noinline__
 inline
 #endif
 void gs_coord_on_ack(double* coord, uint32_t* ctag, double* adj, uint32_t* adj_idx, const uint8_t* imp_delay,
-                     const GsGlobals& g, uint32_t i,
+                     uint32_t on, const GsGlobals& g, uint32_t i,
                      uint32_t j, uint32_t t) {  // (column pointers by value: taking the address of the
                                                  // kernel's GsDev parameter would copy it to the stack)
   const size_t cap = g.cap;
@@ -321,7 +336,8 @@ void gs_coord_on_ack(double* coord, uint32_t* ctag, double* adj, uint32_t* adj_i
   gs_coord_load(coord, cap, mine, i, c);
   gs_coord_load(coord, cap, gs_coord_slot_for_reader(ctag, cap, j, t), j, other);
   const double rtt =
-      g.coord_base_rtt_s + (double)(gs_extra(g, imp_delay, i, j) + gs_extra(g, imp_delay, j, i)) * g.tick_seconds;
+      g.coord_base_rtt_s + (double)(gs_extra(g, imp_delay, i, j, on >> 1) + gs_extra(g, imp_delay, j, i, on & 1u)) *
+                               g.tick_seconds;  // (on: bit 0 = i's delay in force, bit 1 = j's)
   uint32_t idx = adj_idx[i];
   gs_coord_client_update(c, other, rtt, adj + i, cap, &idx, g.seed_lo, g.seed_hi, i, t);
   adj_idx[i] = idx;
@@ -564,9 +580,21 @@ GS_DEV bool gs_mail_is_stale(const GsGlobals& g, uint32_t w, uint32_t heard, boo
 // away, so a pool without any runs the code it would run without the feature.
 // PIG: the pool piggybacks broadcasts on probe traffic (GsDev::pig_req / pig are set); likewise folded away
 // in the other instantiation.
-template <bool IMPAIRED, bool PIG = false, class Sink>
+// FLAP (with IMPAIRED): some impaired member has a flap schedule (GsDev::imp_flap is set); the impaired
+// instantiation without it folds every schedule term away, so impaired pools without schedules run the code
+// they ran before the feature.
+// FLAP: whether member x's impairment is in force at t (gs_imp_on); the row step asks once per member and stage
+// where it is needed, keeping the answers out of long live ranges (it runs at the register limit).  Every other
+// instantiation folds the `on` bits to 1.
+template <bool FLAP>
+GS_DEV uint32_t gs_on(const GsDev& d, const GsGlobals& g, uint32_t x, uint32_t t) {
+  return FLAP ? gs_imp_on(g, d.imp_flap, x, t) : 1u;
+}
+
+template <bool IMPAIRED, bool PIG = false, bool FLAP = false, class Sink>
 GS_DEV void gs_row_step_body(const GsDev& d, const GsGlobals& g, uint32_t i, uint32_t t, uint32_t gslot,
                              uint32_t inb, Sink& sink) {
+  static_assert(IMPAIRED || !FLAP, "a flap schedule gates an impairment");
   const GsLossCols imp_loss = {IMPAIRED ? d.imp_loss : nullptr, IMPAIRED ? d.imp_recv : nullptr};
   const uint8_t* const imp_delay = IMPAIRED ? d.imp_delay : nullptr;
   const uint8_t* const imp_flags = IMPAIRED ? d.imp_flags : nullptr;
@@ -740,7 +768,7 @@ GS_DEV void gs_row_step_body(const GsDev& d, const GsGlobals& g, uint32_t i, uin
           gs_pig_count(d, i, GS_PIG_ST_SERVED, 1u);
           const uint32_t pkt = gs_pig_take(d, g, i, queued, (e >> 1) & 3u);
           if (pkt != 0u && !(e & 1u))
-            gs_post(d, g, sink, (t + 1u + gs_extra(g, imp_delay, i, e >> 3)) & g.ring_mask, e >> 3, pkt);
+            gs_post(d, g, sink, (t + 1u + gs_extra(g, imp_delay, i, e >> 3, gs_on<FLAP>(d, g, e >> 3, t))) & g.ring_mask, e >> 3, pkt);
         }
       }
     }
@@ -794,50 +822,59 @@ GS_DEV void gs_row_step_body(const GsDev& d, const GsGlobals& g, uint32_t i, uin
       const uint32_t budget = g.P * (gs_meta_aw(m) + 1u) - g.T;
       bool pig_gate = false;
       if constexpr (PIG) pig_gate = gs_pig_gate(d, t);
+      const uint32_t on_ij = gs_on<FLAP>(d, g, i, t) | gs_on<FLAP>(d, g, j, t) << 1;  // bit 0: this member, bit 1: the target
       for (uint32_t q = 0; q < nr; ++q) {
         const uint32_t r = relays[q];
+        const uint32_t on_r = gs_on<FLAP>(d, g, r, t);
         const bool r_up = gs_key_truth(gs_peer_key(d, cur, r, false)) == GS_TRUTH_UP;
         sink.stat(GS_ST_INDIRECT_PINGS, 1);
         if constexpr (PIG) {
           // the request carries broadcasts of this member's queue; the relay's ping to j, j's ack and the
           // relay's forwarded ack or nack are owed by whoever sends them (same loss draws as below)
-          const bool req_lost = gs_lost_quiet(g, imp_loss, i, r, t, GS_LK_INDREQ, q);
+          const bool req_lost = gs_lost_quiet(g, imp_loss, i, r, t, GS_LK_INDREQ, q, (on_ij & 1u) | on_r << 1);
           const uint32_t pkt = gs_pig_take(d, g, i, queued, GS_PIG_INDREQ);
-          if (pkt != 0u && !req_lost) gs_post(d, g, sink, (t + 1u + gs_extra(g, imp_delay, i, r)) & g.ring_mask, r, pkt);
+          if (pkt != 0u && !req_lost) gs_post(d, g, sink, (t + 1u + gs_extra(g, imp_delay, i, r, on_r)) & g.ring_mask, r, pkt);
           if (pig_gate && r_up && !req_lost) {
-            const bool ping_lost = gs_lost_quiet(g, imp_loss, r, j, t, GS_LK_INDPING, q);
+            const bool ping_lost = gs_lost_quiet(g, imp_loss, r, j, t, GS_LK_INDPING, q, on_r | (on_ij & 2u));
             gs_pig_owe(d, g, sink, nxt, inxt, r, j, GS_PIG_PING, ping_lost);
-            const bool ack_lost = gs_lost_quiet(g, imp_loss, j, r, t, GS_LK_INDACK, q);
+            const bool ack_lost = gs_lost_quiet(g, imp_loss, j, r, t, GS_LK_INDACK, q, on_ij >> 1 | on_r << 1);
             if (j_up && !ping_lost) gs_pig_owe(d, g, sink, nxt, inxt, j, r, GS_PIG_ACK, ack_lost);
             const bool acked = j_up && !ping_lost && !ack_lost &&
-                               gs_extra(g, imp_delay, r, j) + gs_extra(g, imp_delay, j, r) <= g.T;
+                               gs_extra(g, imp_delay, r, j, on_ij >> 1) + gs_extra(g, imp_delay, j, r, on_r) <= g.T;
             if (acked)
-              gs_pig_owe(d, g, sink, nxt, inxt, r, i, GS_PIG_ACK, gs_lost_quiet(g, imp_loss, r, i, t, GS_LK_INDFWD, q));
+              gs_pig_owe(d, g, sink, nxt, inxt, r, i, GS_PIG_ACK,
+                         gs_lost_quiet(g, imp_loss, r, i, t, GS_LK_INDFWD, q, on_r | (on_ij & 1u) << 1));
             else
-              gs_pig_owe(d, g, sink, nxt, inxt, r, i, GS_PIG_NACK, gs_lost_quiet(g, imp_loss, r, i, t, GS_LK_NACK, q));
+              gs_pig_owe(d, g, sink, nxt, inxt, r, i, GS_PIG_NACK,
+                         gs_lost_quiet(g, imp_loss, r, i, t, GS_LK_NACK, q, on_r | (on_ij & 1u) << 1));
           }
         }
-        if (!(r_up && !gs_lost(g, imp_loss, sink, i, r, t, GS_LK_INDREQ, q))) continue;  // no nack either
-        const uint32_t via = gs_extra(g, imp_delay, i, r) + gs_extra(g, imp_delay, r, i);
-        const uint32_t rtt_rj = gs_extra(g, imp_delay, r, j) + gs_extra(g, imp_delay, j, r);
+        if (!(r_up && !gs_lost(g, imp_loss, sink, i, r, t, GS_LK_INDREQ, q, (on_ij & 1u) | on_r << 1))) continue;  // no nack either
+        const uint32_t via = gs_extra(g, imp_delay, i, r, on_r) + gs_extra(g, imp_delay, r, i, on_ij & 1u);
+        const uint32_t rtt_rj = gs_extra(g, imp_delay, r, j, on_ij >> 1) + gs_extra(g, imp_delay, j, r, on_r);
         // the relay waits ProbeTimeout for the target's ack, then answers with a nack
-        bool relay_acked = j_up && !gs_lost(g, imp_loss, sink, r, j, t, GS_LK_INDPING, q) &&
-                           !gs_lost(g, imp_loss, sink, j, r, t, GS_LK_INDACK, q) && rtt_rj <= g.T;
+        bool relay_acked = j_up && !gs_lost(g, imp_loss, sink, r, j, t, GS_LK_INDPING, q, on_r | (on_ij & 2u)) &&
+                           !gs_lost(g, imp_loss, sink, j, r, t, GS_LK_INDACK, q, on_ij >> 1 | on_r << 1) && rtt_rj <= g.T;
         if (relay_acked) {
-          if (!gs_lost(g, imp_loss, sink, r, i, t, GS_LK_INDFWD, q) && via + rtt_rj <= budget) success = true;
-        } else if (!gs_lost(g, imp_loss, sink, r, i, t, GS_LK_NACK, q) && via <= budget) {
+          if (!gs_lost(g, imp_loss, sink, r, i, t, GS_LK_INDFWD, q, on_r | (on_ij & 1u) << 1) && via + rtt_rj <= budget)
+            success = true;
+        } else if (!gs_lost(g, imp_loss, sink, r, i, t, GS_LK_NACK, q, on_r | (on_ij & 1u) << 1) && via <= budget) {
           ++nacks;
           sink.stat(GS_ST_NACKS, 1);
         }
       }
       const uint32_t t0 = t - g.T;
-      const uint32_t rtt_ij = gs_extra(g, imp_delay, i, j) + gs_extra(g, imp_delay, j, i);
+      const uint32_t rtt_ij = gs_extra(g, imp_delay, i, j, on_ij >> 1) + gs_extra(g, imp_delay, j, i, on_ij & 1u);
       // TCP fallback ping: reliable, unless either end has TCP blocked (GSIM_IMPAIR_NO_TCP)
-      if (!g.disable_tcp && j_up && rtt_ij <= budget && !gs_no_tcp(imp_flags, i, j)) success = true;
-      // a direct ack that was merely slower than ProbeTimeout still counts until the deadline
-      if ((g.n_dcs != 0u || imp_delay != nullptr) && j_up && rtt_ij > g.T && rtt_ij <= budget + g.T &&
-          !gs_lost_quiet(g, imp_loss, i, j, t0, GS_LK_PING, 0) && !gs_lost_quiet(g, imp_loss, j, i, t0, GS_LK_ACK, 0))
-        success = true;
+      if (!g.disable_tcp && j_up && rtt_ij <= budget && !gs_no_tcp(imp_flags, i, j, on_ij)) success = true;
+      // a direct ack that was merely slower than ProbeTimeout still counts until the deadline (its loss draws
+      // are the probe's, at t0, and so are the ends' schedules)
+      if ((g.n_dcs != 0u || imp_delay != nullptr) && j_up && rtt_ij > g.T && rtt_ij <= budget + g.T) {
+        const uint32_t on0 = FLAP ? gs_imp_on(g, d.imp_flap, i, t0) | gs_imp_on(g, d.imp_flap, j, t0) << 1 : 3u;
+        if (!gs_lost_quiet(g, imp_loss, i, j, t0, GS_LK_PING, 0, on0) &&
+            !gs_lost_quiet(g, imp_loss, j, i, t0, GS_LK_ACK, 0, on0 >> 1 | (on0 & 1u) << 1))
+          success = true;
+      }
       if (success) {
         uint32_t aw = gs_meta_aw(m);
         m = gs_meta_set_aw(m, aw ? aw - 1u : 0u);
@@ -904,25 +941,27 @@ GS_DEV void gs_row_step_body(const GsDev& d, const GsGlobals& g, uint32_t i, uin
       d.pass[i] = pass;
       if (target != GS_EMPTY32) {
         sink.stat(GS_ST_PROBES, 1);
+        const uint32_t on_it = gs_on<FLAP>(d, g, i, t) | gs_on<FLAP>(d, g, target, t) << 1;  // bit 0: this member, bit 1: the target
         if constexpr (PIG) {
           // the ping carries broadcasts of this member's queue; the target owes its ack (same loss draws as below)
-          const bool ping_lost = gs_lost_quiet(g, imp_loss, i, target, t, GS_LK_PING, 0);
+          const bool ping_lost = gs_lost_quiet(g, imp_loss, i, target, t, GS_LK_PING, 0, on_it);
           const uint32_t pkt = gs_pig_take(d, g, i, queued, GS_PIG_PING);
           if (pkt != 0u && !ping_lost)
-            gs_post(d, g, sink, (t + 1u + gs_extra(g, imp_delay, i, target)) & g.ring_mask, target, pkt);
+            gs_post(d, g, sink, (t + 1u + gs_extra(g, imp_delay, i, target, on_it >> 1)) & g.ring_mask, target, pkt);
           if (gs_pig_gate(d, t) && gs_key_truth(ktarget) == GS_TRUTH_UP && !ping_lost)
-            gs_pig_owe(d, g, sink, nxt, inxt, target, i, GS_PIG_ACK, gs_lost_quiet(g, imp_loss, target, i, t, GS_LK_ACK, 0));
+            gs_pig_owe(d, g, sink, nxt, inxt, target, i, GS_PIG_ACK,
+                       gs_lost_quiet(g, imp_loss, target, i, t, GS_LK_ACK, 0, on_it >> 1 | (on_it & 1u) << 1));
         }
-        bool ok = gs_key_truth(ktarget) == GS_TRUTH_UP && !gs_lost(g, imp_loss, sink, i, target, t, GS_LK_PING, 0) &&
-                  !gs_lost(g, imp_loss, sink, target, i, t, GS_LK_ACK, 0) &&
-                  gs_extra(g, imp_delay, i, target) + gs_extra(g, imp_delay, target, i) <= g.T;  // ack within ProbeTimeout
+        bool ok = gs_key_truth(ktarget) == GS_TRUTH_UP && !gs_lost(g, imp_loss, sink, i, target, t, GS_LK_PING, 0, on_it) &&
+                  !gs_lost(g, imp_loss, sink, target, i, t, GS_LK_ACK, 0, on_it >> 1 | (on_it & 1u) << 1) &&
+                  gs_extra(g, imp_delay, i, target, on_it >> 1) + gs_extra(g, imp_delay, target, i, on_it & 1u) <= g.T;  // ack within ProbeTimeout
         if (ok) {
           uint32_t aw = gs_meta_aw(m);
           m = gs_meta_set_aw(m, aw ? aw - 1u : 0u);
           due = t + g.P;
           sink.stat(GS_ST_ACKS, 1);
           if constexpr (Sink::kCoords) {  // the ack carries the peer's coordinate
-            if (d.coord != nullptr) gs_coord_on_ack(d.coord, d.ctag, d.adj, d.adj_idx, imp_delay, g, i, target, t);
+            if (d.coord != nullptr) gs_coord_on_ack(d.coord, d.ctag, d.adj, d.adj_idx, imp_delay, on_it, g, i, target, t);
           }
         } else {
           m = gs_meta_set_stage(m, GS_STAGE_WAIT_T);
@@ -1003,8 +1042,9 @@ GS_DEV void gs_row_step_body(const GsDev& d, const GsGlobals& g, uint32_t i, uin
               pm &= pm - 1;
               if (((sends >> (4u * x)) & 15u) > q) pkt |= 1u << r;
             }
-            if (!gs_lost(g, imp_loss, sink, i, peers[q], t, GS_LK_GOSSIP, q))
-              gs_post(d, g, sink, (t + 1u + gs_extra(g, imp_delay, i, peers[q])) & g.ring_mask, peers[q], pkt);
+            const uint32_t on_p = gs_on<FLAP>(d, g, peers[q], t);
+            if (!gs_lost(g, imp_loss, sink, i, peers[q], t, GS_LK_GOSSIP, q, gs_on<FLAP>(d, g, i, t) | on_p << 1))
+              gs_post(d, g, sink, (t + 1u + gs_extra(g, imp_delay, i, peers[q], on_p)) & g.ring_mask, peers[q], pkt);
           }
           np = 0u;  // done: the general loop below has nothing left to do
         }
@@ -1026,8 +1066,9 @@ GS_DEV void gs_row_step_body(const GsDev& d, const GsGlobals& g, uint32_t i, uin
           sink.stat(GS_ST_RUMORS_SENT, 1);
         }
         sink.stat(GS_ST_GOSSIP_PACKETS, 1);
-        if (!gs_lost(g, imp_loss, sink, i, peers[q], t, GS_LK_GOSSIP, q))
-          gs_post(d, g, sink, (t + 1u + gs_extra(g, imp_delay, i, peers[q])) & g.ring_mask, peers[q], pkt);
+        const uint32_t on_p = gs_on<FLAP>(d, g, peers[q], t);
+        if (!gs_lost(g, imp_loss, sink, i, peers[q], t, GS_LK_GOSSIP, q, gs_on<FLAP>(d, g, i, t) | on_p << 1))
+          gs_post(d, g, sink, (t + 1u + gs_extra(g, imp_delay, i, peers[q], on_p)) & g.ring_mask, peers[q], pkt);
       }
       if (queued != q0) d.queued[i] = queued;
     }
@@ -1042,7 +1083,7 @@ GS_DEV void gs_row_step_body(const GsDev& d, const GsGlobals& g, uint32_t i, uin
         const uint32_t j = partner[0];
         // an end that cannot use TCP (GSIM_IMPAIR_NO_TCP): the exchange is started and counted, but
         // nothing is pushed and nothing comes back
-        if (!gs_no_tcp(imp_flags, i, j)) {
+        if (!gs_no_tcp(imp_flags, i, j, gs_on<FLAP>(d, g, i, t) | gs_on<FLAP>(d, g, j, t) << 1)) {
           uint32_t* req = d.ppreq + (size_t)nxt * GS_PPK * cap;
           uint32_t v = i;
           for (uint32_t s = 0; s < GS_PPK; ++s) {
@@ -1087,11 +1128,13 @@ template <class Sink>
 GS_DEV void gs_row_step(const GsDev& d, const GsGlobals& g, uint32_t i, uint32_t t, uint32_t gslot, uint32_t inb,
                         Sink& sink) {
   if (d.pig != nullptr) {
-    if (d.imp_loss != nullptr) gs_row_step_body<true, true>(d, g, i, t, gslot, inb, sink);
+    if (d.imp_flap != nullptr) gs_row_step_body<true, true, true>(d, g, i, t, gslot, inb, sink);
+    else if (d.imp_loss != nullptr) gs_row_step_body<true, true>(d, g, i, t, gslot, inb, sink);
     else gs_row_step_body<false, true>(d, g, i, t, gslot, inb, sink);
     return;
   }
-  if (d.imp_loss != nullptr) gs_row_step_body<true>(d, g, i, t, gslot, inb, sink);
+  if (d.imp_flap != nullptr) gs_row_step_body<true, false, true>(d, g, i, t, gslot, inb, sink);
+  else if (d.imp_loss != nullptr) gs_row_step_body<true>(d, g, i, t, gslot, inb, sink);
   else gs_row_step_body<false>(d, g, i, t, gslot, inb, sink);
 }
 

@@ -294,6 +294,31 @@ class Pool:
                                               C.byref(flags)))
         return send.value, recv.value, delay.value, bool(flags.value & IMPAIR_NO_TCP)
 
+    def impair_flap(self, ids, period_ticks: int, bad_ppm: int):
+        """Make the impairment of the listed members intermittent: in force only during bad epochs of
+        `period_ticks` ticks, each bad with probability bad_ppm / 1e6.  period_ticks 0 clears the schedule
+        (impairment always in force)."""
+        arr = (C.c_uint32 * max(1, len(ids)))(*ids)
+        self._ck(self.lib.gsim_impair_flap_many(self.h, arr, len(ids), period_ticks, bad_ppm))
+
+    def impair_flap_fraction(self, member_ppm: int, salt: int, period_ticks: int, bad_ppm: int) -> int:
+        """impair_flap on the members impair_fraction selects for the same salt; returns how many."""
+        out = C.c_uint32()
+        self._ck(self.lib.gsim_impair_flap_fraction(self.h, member_ppm, salt, period_ticks, bad_ppm, C.byref(out)))
+        return out.value
+
+    def impair_flap_get(self, member: int):
+        """(period_ticks, bad_ppm) of one member's schedule, (0, 0) without one."""
+        period, ppm = C.c_uint32(), C.c_uint32()
+        self._ck(self.lib.gsim_impair_flap_get(self.h, member, C.byref(period), C.byref(ppm)))
+        return period.value, ppm.value
+
+    def flap_stats(self):
+        """{'scheduled', 'bad'}: members with a schedule, and those of them in a bad epoch now."""
+        out = (C.c_uint64 * 2)()
+        self._ck(self.lib.gsim_impair_flap_stats(self.h, out))
+        return {"scheduled": out[0], "bad": out[1]}
+
     def pause(self, ids, ticks: int) -> int:
         """Stop the listed members (running, not leaving) for `ticks` ticks; returns how many were paused."""
         arr = (C.c_uint32 * max(1, len(ids)))(*ids)

@@ -375,6 +375,39 @@ int gsim_impair_dir_fraction(gsim_pool* p, uint32_t member_ppm, uint32_t salt, u
 int gsim_impair_dir_get(gsim_pool* p, uint32_t id, uint32_t* send_loss_ppm, uint32_t* recv_loss_ppm,
                         uint32_t* delay_ticks, uint32_t* flags);
 
+/* Intermittent impairment (DESIGN.md §3.5 "Intermittent impairment"): a member with a flap schedule
+ * (period_ticks, bad_ppm) has its impairment (the four gsim_impair_dir_get values) in force only during bad
+ * epochs; in a good epoch it behaves as if all four were 0.  A member without a schedule behaves as before.
+ *  - phase(m) = philox(seed; m, 0xFFFFFFFF, FLAP = 12).y mod period; epoch(m, t) = (t + phase(m)) / period in
+ *    64 bits; bad(m, t) iff philox(seed; m, epoch(m, t), FLAP).x < bad_ppm * 2^32 / 1e6 (the ppm threshold of
+ *    gsim_crash_fraction), and always for bad_ppm = 1e6.  gsim_flap_bad is this function.
+ *  - Which tick: a packet src -> dst sent at t uses bad(src, t) for the send threshold and bad(dst, t) for
+ *    the receive threshold and delay; GSIM_IMPAIR_NO_TCP applies to an end that is bad at the tick of the
+ *    exchange; gsim_join and the true_s of gsim_rtt_many use gsim_now.
+ *  - Unchanged: accusations, wake bits and host operations stay lossless.  The probe fast paths, quiet
+ *    windows and gsim_health_histogram go by the static values: a schedule turns none of them on or off,
+ *    and a schedule on a member whose four values are 0 has no effect.
+ *  - Column: 4 bytes per member, allocated by the first schedule call; members added later start without a
+ *    schedule.  The schedule is configuration: not part of gsim_state_hash; gsim_snapshot carries it.
+ *  - Errors: GSIM_ERR_INVALID for period_ticks > 4095, bad_ppm > 1e6 or member_ppm > 1e6;
+ *    GSIM_ERR_NOT_FOUND for an id never created; GSIM_ERR_STATE on a sharded pool. */
+#define GSIM_FLAP_MAX_PERIOD 4095u
+/* Give the listed members the schedule (period_ticks 1..4095, bad_ppm <= 1e6); period_ticks 0 clears it
+ * (impairment always in force, as before). */
+int gsim_impair_flap_many(gsim_pool* p, const uint32_t* ids, size_t n, uint32_t period_ticks, uint32_t bad_ppm);
+/* The selection of gsim_impair_fraction (the same salt picks the same members); *n_selected = members selected. */
+int gsim_impair_flap_fraction(gsim_pool* p, uint32_t member_ppm, uint32_t salt, uint32_t period_ticks,
+                              uint32_t bad_ppm, uint32_t* n_selected);
+/* The schedule of member `id`, (0, 0) without one. */
+int gsim_impair_flap_get(gsim_pool* p, uint32_t id, uint32_t* period_ticks, uint32_t* bad_ppm);
+/* out = {members with a schedule, of those the ones in a bad epoch at gsim_now}; read-only, one device
+ * submission. */
+int gsim_impair_flap_stats(gsim_pool* p, uint64_t out[2]);
+/* The pure schedule function (for known-answer tests, like gsim_ring_entry): 1 if `member` is in a bad epoch at
+ * `tick` under (period_ticks, bad_ppm) with pool seed `seed`, else 0; 1 for period_ticks 0 (no schedule: the
+ * impairment is always in force); GSIM_ERR_INVALID for out-of-range arguments. */
+int gsim_flap_bad(uint64_t seed, uint32_t member, uint32_t period_ticks, uint32_t bad_ppm, uint32_t tick);
+
 /* Paused members (simulator-only fault injection: a GC pause, a VM steal, a SIGSTOP; DESIGN.md §3.6):
  * a member paused at tick t0 for d ticks is a stopped process during ticks t0 .. t0+d-1 and carries on
  * with the state it had at t0+d.
