@@ -131,6 +131,16 @@ SIGNATURES = [
     ("gsim_impair_flap_get", _i32, [_P, _u32, C.POINTER(_u32), C.POINTER(_u32)]),
     ("gsim_impair_flap_stats", _i32, [_P, C.POINTER(_u64)]),
     ("gsim_flap_bad", _i32, [_u64, _u32, _u32, _u32, _u32]),
+    ("gsim_domain_set_many", _i32, [_P, C.POINTER(_u32), _sz, _u32]),
+    ("gsim_domain_set_range", _i32, [_P, _u32, _u32, _u32, _u32]),
+    ("gsim_domain_get", _i32, [_P, _u32, _u32, _P]),
+    ("gsim_domain_flap_set", _i32, [_P, C.POINTER(_u32), _sz, _u32, _u32]),
+    ("gsim_domain_flap_get", _i32, [_P, _u32, C.POINTER(_u32), C.POINTER(_u32)]),
+    ("gsim_domain_flap_bad", _i32, [_u64, _u32, _u32, _u32, _u32]),
+    ("gsim_domain_impair", _i32, [_P, C.POINTER(_u32), _sz, _u32, _u32, _u32, _u32, C.POINTER(_u32)]),
+    ("gsim_domain_crash", _i32, [_P, C.POINTER(_u32), _sz, C.POINTER(_u32)]),
+    ("gsim_domain_pause", _i32, [_P, C.POINTER(_u32), _sz, _u32, C.POINTER(_u32)]),
+    ("gsim_domain_stats_read", _i32, [_P, _u32, _u32, _P]),
     ("gsim_pause_many", _i32, [_P, C.POINTER(_u32), _sz, _u32, C.POINTER(_u32)]),
     ("gsim_pause_fraction", _i32, [_P, _u32, _u32, _u32, C.POINTER(_u32)]),
     ("gsim_pause_get", _i32, [_P, _u32, C.POINTER(_u32)]),

@@ -307,6 +307,15 @@ struct gsim_pool {
   // the column only while that count and n_impaired are > 0 (a schedule gates an impairment).
   uint32_t* imp_flap = nullptr;
   uint32_t n_flap = 0;
+  // ... and fault domains (gsim_domain_*): the domain column (0 = none), allocated by the first domain call;
+  // the domain schedule table, dom_tab[x] = gs_flap_word of domain x (0 = none), as long as the highest id
+  // ever given a schedule, with its device copy (dom_tab_cap entries) and how many entries are non-zero.
+  // d.imp_dom / d.dom_flap point at them only while that count and n_impaired are > 0.
+  uint32_t* imp_dom = nullptr;
+  std::vector<uint32_t> dom_tab;
+  uint32_t* dom_tab_dev = nullptr;
+  size_t dom_tab_cap = 0;
+  uint32_t n_dom_sched = 0;
   // paused members (gsim_pause_*): the resume-tick column (0 = not paused) and {paused now, resumed Alive,
   // Suspect, Dead}; the first pause allocates the column and pause_cnt_dev, a device copy of the counts that
   // exists only so that snapshots carry them
@@ -1284,14 +1293,17 @@ extern "C" int gsim_join(gsim_pool* p, uint32_t id, const uint32_t* seeds, size_
   uint32_t* ri = row(id);
   if (gs_key_truth(ri[cur]) != GS_TRUTH_UP) return fail(p, GSIM_ERR_STATE, "member is not running");
   // GSIM_IMPAIR_NO_TCP at the joiner or at a seed: the push-pull to that seed cannot connect (only pools
-  // that have the flag column read it; a member with a flap schedule only while it is in a bad epoch now)
+  // that have the flag column read it; a member with a flap schedule of its own or of its domain only while
+  // its impairment is in force now, gs_in_force)
   std::vector<uint8_t> no_tcp(ids.size(), 0u);
   for (size_t x = 0; p->imp_flags && x < ids.size(); ++x) {
     if (!peek(p, p->imp_flags, ids[x], &no_tcp[x])) return fail(p, GSIM_ERR_CUDA, "peek");
     no_tcp[x] &= GSIM_IMPAIR_NO_TCP;
-    uint32_t w = 0u;
+    uint32_t w = 0u, dom = 0u, wd = 0u;
     if (no_tcp[x] && p->d.imp_flap && !peek(p, p->imp_flap, ids[x], &w)) return fail(p, GSIM_ERR_CUDA, "peek");
-    if (w != 0u && !gs_flap_bad(g.seed_lo, g.seed_hi, ids[x], w, p->now)) no_tcp[x] = 0u;
+    if (no_tcp[x] && p->d.dom_flap && !peek(p, p->imp_dom, ids[x], &dom)) return fail(p, GSIM_ERR_CUDA, "peek");
+    if (p->d.dom_flap && dom < p->dom_tab.size()) wd = p->dom_tab[dom];
+    if (!gs_in_force(g.seed_lo, g.seed_hi, ids[x], w, dom, wd, p->now)) no_tcp[x] = 0u;
   }
   auto tcp_blocked = [&](uint32_t m) { return no_tcp[std::find(ids.begin(), ids.end(), m) - ids.begin()] != 0u; };
   int okc = 0;
@@ -1712,7 +1724,7 @@ struct HostCoords {
   std::vector<double> coord;
   std::vector<uint32_t> ctag, key;
   std::vector<uint8_t> delay;
-  std::vector<uint32_t> flap;
+  std::vector<uint32_t> flap, dom, dom_flap;
   GsDev d;
   bool load(GsBackend* be, const GsDev& dd, const GsGlobals& g, uint32_t now, bool keys) {
     const size_t cap = g.cap;
@@ -1732,6 +1744,14 @@ struct HostCoords {
       flap.resize(cap);
       if (!be->d2h(flap.data(), dd.imp_flap, cap * 4)) return false;
       d.imp_flap = flap.data();
+    }
+    if (dd.dom_flap) {
+      dom.resize(cap);
+      dom_flap.resize(dd.dom_flap_n);
+      if (!be->d2h(dom.data(), dd.imp_dom, cap * 4) || !be->d2h(dom_flap.data(), dd.dom_flap, (size_t)dd.dom_flap_n * 4))
+        return false;
+      d.imp_dom = dom.data();
+      d.dom_flap = dom_flap.data();
     }
     if (keys) {
       key.resize(g.n);
@@ -1767,7 +1787,7 @@ bool GsBackend::coord_pairs(const GsDev& d, const GsGlobals*, const GsGlobals& g
     gs_coord_pick(h.d.coord, h.d.ctag, g.cap, ha[k], ca);
     gs_coord_pick(h.d.coord, h.d.ctag, g.cap, hb[k], cb);
     he[k] = gs_coord_distance_seconds(ca, cb);
-    ht[k] = gs_model_rtt(g, h.d.imp_delay, h.d.imp_flap, ha[k], hb[k], now);
+    ht[k] = gs_model_rtt(g, h.d, ha[k], hb[k], now);
   }
   return h2d(est, he.data(), (size_t)n * 8) && (!tru || h2d(tru, ht.data(), (size_t)n * 8));
 }
@@ -2107,6 +2127,10 @@ static void impair_publish(gsim_pool* p) {
   p->d.imp_recv = p->n_impaired ? (p->imp_recv ? p->imp_recv : p->imp_loss) : nullptr;
   p->d.imp_flags = p->n_impaired ? p->imp_flags : nullptr;
   p->d.imp_flap = p->n_impaired && p->n_flap ? p->imp_flap : nullptr;
+  const bool dom_on = p->n_impaired && p->n_dom_sched;
+  p->d.imp_dom = dom_on ? p->imp_dom : nullptr;
+  p->d.dom_flap = dom_on ? p->dom_tab_dev : nullptr;
+  p->d.dom_flap_n = dom_on ? (uint32_t)p->dom_tab.size() : 0u;
   mark_dirty(p);
 }
 
@@ -2376,7 +2400,7 @@ struct HostRows {
     key0.resize(n), key1.resize(n), meta.resize(n), due.resize(n), inbox.resize(n), pause.resize(n);
     if (!be->d2h(key0.data(), dd.key[0], n * 4) || !be->d2h(key1.data(), dd.key[1], n * 4) ||
         !be->d2h(meta.data(), dd.meta, n * 4) || !be->d2h(due.data(), dd.due, n * 4) ||
-        !be->d2h(inbox.data(), dd.inbox[slot], n * 4) || !be->d2h(pause.data(), pause_until, n * 4))
+        !be->d2h(inbox.data(), dd.inbox[slot], n * 4) || (pause_until && !be->d2h(pause.data(), pause_until, n * 4)))
       return false;
     if (dd.kst) {
       kst.resize(n);
@@ -2394,7 +2418,7 @@ struct HostRows {
     const size_t n = g.n;
     return be->h2d(dd.key[0], key0.data(), n * 4) && be->h2d(dd.key[1], key1.data(), n * 4) &&
            be->h2d(dd.meta, meta.data(), n * 4) && be->h2d(dd.due, due.data(), n * 4) &&
-           be->h2d(dd.inbox[slot], inbox.data(), n * 4) && be->h2d(pause_until, pause.data(), n * 4) &&
+           be->h2d(dd.inbox[slot], inbox.data(), n * 4) && (!pause_until || be->h2d(pause_until, pause.data(), n * 4)) &&
            (!dd.kst || be->h2d(dd.kst, kst.data(), n));
   }
 };
@@ -2462,6 +2486,8 @@ static int pause_check(gsim_pool* p, uint32_t ticks) {
   return GSIM_OK;
 }
 
+static int pause_done(gsim_pool* p, uint32_t until, uint32_t k, uint32_t* n_paused);
+
 // The selected members (ids[0..n), or the draw below thr) stop now and resume at now + ticks: one resume
 // entry in the schedule per distinct tick, which also makes gsim_step end its chunks (windows, tick
 // stretches) there.
@@ -2474,6 +2500,11 @@ static int pause_run(gsim_pool* p, const uint32_t* ids, uint32_t n, uint32_t thr
   uint32_t k = 0;
   if (!dev(p)->pause_rows(p->d, p->g_dev, p->g, p->pause_until, ids, n, thr, salt, until, &k))
     return fail(p, GSIM_ERR_CUDA, "pause_rows");
+  return pause_done(p, until, k, n_paused);
+}
+
+// After k members were paused until tick `until`: the counts, the resume entry and the recount.
+static int pause_done(gsim_pool* p, uint32_t until, uint32_t k, uint32_t* n_paused) {
   *n_paused = k;
   if (!k) return GSIM_OK;
   p->pause_cnt[0] += k;
@@ -2546,6 +2577,316 @@ extern "C" int gsim_pause_stats(gsim_pool* p, uint64_t out[4]) {
   if (!p || !out) return GSIM_ERR_INVALID;
   std::lock_guard<std::mutex> lk(p->mu);
   memcpy(out, p->pause_cnt, sizeof(p->pause_cnt));
+  return GSIM_OK;
+}
+
+// ---- fault domains (DESIGN.md §3.5 "Fault domains") -------------------------------------------------
+// The backend defaults (gs_backend.h): the columns the rows read and write, copied to the host, stepped there
+// and copied back.
+bool GsBackend::domain_range(uint32_t* dom, uint32_t first, uint32_t count, uint32_t per_domain, uint32_t first_domain) {
+  if (!count) return true;
+  std::vector<uint32_t> v(count);
+  for (uint32_t x = 0; x < count; ++x) v[x] = first_domain + x / per_domain;
+  return h2d(dom + first, v.data(), (size_t)count * 4);
+}
+
+bool GsBackend::domain_rows(const GsDev& d, const GsGlobals*, const GsGlobals& g, const uint32_t* dom,
+                            const uint32_t* bits, uint32_t n_words, const GsDomainOp& a, uint32_t counts[2]) {
+  counts[0] = counts[1] = 0u;
+  if (!g.n) return true;
+  std::vector<uint32_t> dc(g.n);
+  if (!d2h(dc.data(), dom, (size_t)g.n * 4)) return false;
+  GsDomainOp ha = a;
+  HostRows h;
+  std::vector<uint32_t> lc, rc;
+  std::vector<uint8_t> delay, fc;
+  if (a.op == GS_DOMAIN_OP_IMPAIR) {
+    lc.resize(g.n), delay.resize(g.n), rc.resize(a.imp.recv ? g.n : 0u), fc.resize(a.imp.flags ? g.n : 0u);
+    if (!d2h(lc.data(), a.imp.loss, (size_t)g.n * 4) || !d2h(delay.data(), a.imp.delay, g.n) ||
+        (a.imp.recv && !d2h(rc.data(), a.imp.recv, (size_t)g.n * 4)) || (a.imp.flags && !d2h(fc.data(), a.imp.flags, g.n)))
+      return false;
+    ha.imp = {lc.data(), a.imp.recv ? rc.data() : nullptr, delay.data(), a.imp.flags ? fc.data() : nullptr};
+  } else if (a.op != GS_DOMAIN_OP_COUNT) {
+    if (!h.load(this, d, g, a.pause_until, 0u)) return false;
+    ha.pause_until = a.pause_until ? h.pause.data() : nullptr;
+  }
+  for (uint32_t i = 0; i < g.n; ++i) {
+    if (!gs_domain_listed(dc.data(), bits, n_words, i)) continue;
+    const uint32_t r = gs_domain_op_row(h.d, g, ha, i);
+    counts[0] += r & 1u;
+    counts[1] += (r >> 1) & 1u;
+  }
+  if (a.op == GS_DOMAIN_OP_IMPAIR)
+    return h2d(a.imp.loss, lc.data(), (size_t)g.n * 4) && h2d(a.imp.delay, delay.data(), g.n) &&
+           (!a.imp.recv || h2d(a.imp.recv, rc.data(), (size_t)g.n * 4)) && (!a.imp.flags || h2d(a.imp.flags, fc.data(), g.n));
+  return a.op == GS_DOMAIN_OP_COUNT || h.store(this, d, g, a.pause_until);
+}
+
+bool GsBackend::domain_stats(const GsDev& d, const GsGlobals& g, const GsDomainCols& c, uint32_t now,
+                             uint32_t first_domain, uint32_t count, GsDomainStats* out) {
+  memset(out, 0, (size_t)count * sizeof(GsDomainStats));
+  if (!g.n || !count) return true;
+  const size_t n = g.n;
+  std::vector<uint32_t> key(n), meta(n), dom(n), pause(c.pause_until ? n : 0u), loss(c.imp.loss ? n : 0u),
+      recv(c.imp.recv ? n : 0u);
+  std::vector<uint8_t> delay(c.imp.delay ? n : 0u), flags(c.imp.flags ? n : 0u);
+  if (!d2h(key.data(), c.key, n * 4) || !d2h(meta.data(), c.meta, n * 4) || !d2h(dom.data(), c.dom, n * 4) ||
+      (c.pause_until && !d2h(pause.data(), c.pause_until, n * 4)) || (c.imp.loss && !d2h(loss.data(), c.imp.loss, n * 4)) ||
+      (c.imp.recv && !d2h(recv.data(), c.imp.recv, n * 4)) || (c.imp.delay && !d2h(delay.data(), c.imp.delay, n)) ||
+      (c.imp.flags && !d2h(flags.data(), c.imp.flags, n)))
+    return false;
+  HostCoords hc;  // the published schedule columns gs_imp_in_force reads
+  hc.d = d;
+  if (d.imp_flap) {
+    hc.flap.resize(g.cap);
+    if (!d2h(hc.flap.data(), d.imp_flap, (size_t)g.cap * 4)) return false;
+    hc.d.imp_flap = hc.flap.data();
+  }
+  if (d.dom_flap) {
+    hc.dom_flap.resize(d.dom_flap_n);
+    if (!d2h(hc.dom_flap.data(), d.dom_flap, (size_t)d.dom_flap_n * 4)) return false;
+    hc.d.imp_dom = dom.data();
+    hc.d.dom_flap = hc.dom_flap.data();
+  }
+  const GsDomainCols h = {key.data(), meta.data(), dom.data(), c.pause_until ? pause.data() : nullptr,
+                          {c.imp.loss ? loss.data() : nullptr, c.imp.recv ? recv.data() : nullptr,
+                           c.imp.delay ? delay.data() : nullptr, c.imp.flags ? flags.data() : nullptr}};
+  for (uint32_t i = 0; i < g.n; ++i) {
+    const uint32_t x = dom[i] - first_domain;
+    uint32_t v[3];
+    if (x >= count || !gs_domain_stats_row(hc.d, g.seed_lo, g.seed_hi, h, i, now, v)) continue;
+    gs_domain_stats_add(out[x], v, v[2]);
+  }
+  return true;
+}
+
+static_assert(sizeof(GsDomainStats) == sizeof(gsim_domain_stats), "GsDomainStats is gsim_domain_stats field for field");
+
+static int domain_sharded(gsim_pool* p) {
+  return fail(p, GSIM_ERR_STATE, "fault domains are not supported on sharded pools");
+}
+
+static bool domain_alloc(gsim_pool* p) {
+  if (p->imp_dom) return true;
+  uint32_t* col = nullptr;
+  if (!alloc_col(p, &col, p->g.cap) || !dev(p)->fill32(col, 0u, p->g.cap)) return false;
+  p->imp_dom = col;
+  return true;
+}
+
+// The device copy of the schedule table, reallocated when the table outgrows it.
+static bool domain_tab_upload(gsim_pool* p) {
+  if (p->dom_tab.size() > p->dom_tab_cap) {
+    size_t cap = p->dom_tab_cap ? p->dom_tab_cap : 1024u;
+    while (cap < p->dom_tab.size()) cap *= 2u;
+    uint32_t* t = nullptr;
+    if (!alloc_col(p, &t, cap)) return false;
+    if (p->dom_tab_dev) {
+      if (!dev(p)->sync()) return false;  // no launch still reads the old copy
+      p->allocs.erase(std::find(p->allocs.begin(), p->allocs.end(), (void*)p->dom_tab_dev));
+      dev(p)->release(p->dom_tab_dev);
+    }
+    p->dom_tab_dev = t;
+    p->dom_tab_cap = cap;
+  }
+  p->n_dom_sched = 0;
+  for (uint32_t w : p->dom_tab) p->n_dom_sched += w != 0u ? 1u : 0u;
+  if (!p->dom_tab.empty() && !dev(p)->h2d(p->dom_tab_dev, p->dom_tab.data(), p->dom_tab.size() * 4)) return false;
+  impair_publish(p);
+  return true;
+}
+
+// A domain list: every id in 1 .. GS_DOMAIN_MAX, as a bitmap (bit x & 31 of word x >> 5).
+static int domain_bits(gsim_pool* p, const uint32_t* domains, size_t n, std::vector<uint32_t>* bits) {
+  uint32_t hi = 0;
+  for (size_t x = 0; x < n; ++x) {
+    if (domains[x] == 0u || domains[x] > GS_DOMAIN_MAX) return fail(p, GSIM_ERR_INVALID, "domain ids are 1 .. GSIM_DOMAIN_MAX");
+    hi = std::max(hi, domains[x]);
+  }
+  bits->assign(n ? hi / 32u + 1u : 0u, 0u);
+  for (size_t x = 0; x < n; ++x) (*bits)[domains[x] >> 5] |= 1u << (domains[x] & 31u);
+  return GSIM_OK;
+}
+
+// One domain operation over the members of the listed domains (none on a pool without a domain column).
+static int domain_run(gsim_pool* p, const std::vector<uint32_t>& bits, const GsDomainOp& a, uint32_t counts[2]) {
+  counts[0] = counts[1] = 0u;
+  if (!p->imp_dom || bits.empty()) return GSIM_OK;
+  if (!upload_globals(p)) return fail(p, GSIM_ERR_CUDA, "upload");
+  if (a.op != GS_DOMAIN_OP_COUNT) mark_dirty(p);
+  if (!dev(p)->domain_rows(p->d, p->g_dev, p->g, p->imp_dom, bits.data(), (uint32_t)bits.size(), a, counts))
+    return fail(p, GSIM_ERR_CUDA, "domain_rows");
+  return GSIM_OK;
+}
+
+extern "C" int gsim_domain_set_many(gsim_pool* p, const uint32_t* ids, size_t n, uint32_t domain) {
+  if (!p || (!ids && n)) return GSIM_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(p->mu);
+  if (p->sharded) return domain_sharded(p);
+  if (domain > GS_DOMAIN_MAX) return fail(p, GSIM_ERR_INVALID, "domain must be <= GSIM_DOMAIN_MAX");
+  for (size_t x = 0; x < n; ++x)
+    if (ids[x] >= p->g.n) return fail(p, GSIM_ERR_NOT_FOUND, "unknown member");
+  if (!domain_alloc(p)) return fail(p, GSIM_ERR_NOMEM, "domain column");
+  for (size_t x = 0; x < n; ++x)
+    if (!poke(p, p->imp_dom, ids[x], domain)) return fail(p, GSIM_ERR_CUDA, "poke");
+  mark_dirty(p);
+  return GSIM_OK;
+}
+
+extern "C" int gsim_domain_set_range(gsim_pool* p, uint32_t first, uint32_t count, uint32_t per_domain,
+                                     uint32_t first_domain) {
+  if (!p) return GSIM_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(p->mu);
+  if (p->sharded) return domain_sharded(p);
+  if (per_domain == 0u) return fail(p, GSIM_ERR_INVALID, "per_domain must be >= 1");
+  if (first_domain == 0u || (count && (uint64_t)first_domain + (count - 1u) / per_domain > GS_DOMAIN_MAX))
+    return fail(p, GSIM_ERR_INVALID, "the domains must lie in 1 .. GSIM_DOMAIN_MAX");
+  if ((uint64_t)first + count > p->g.n) return fail(p, GSIM_ERR_NOT_FOUND, "unknown member");
+  if (!domain_alloc(p)) return fail(p, GSIM_ERR_NOMEM, "domain column");
+  if (!dev(p)->domain_range(p->imp_dom, first, count, per_domain, first_domain)) return fail(p, GSIM_ERR_CUDA, "domain_range");
+  mark_dirty(p);
+  return GSIM_OK;
+}
+
+extern "C" int gsim_domain_get(gsim_pool* p, uint32_t first, uint32_t count, uint32_t* out) {
+  if (!p || (!out && count)) return GSIM_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(p->mu);
+  if (p->sharded) return domain_sharded(p);
+  if ((uint64_t)first + count > p->g.n) return fail(p, GSIM_ERR_NOT_FOUND, "unknown member");
+  if (!p->imp_dom) {
+    memset(out, 0, (size_t)count * 4);
+    return GSIM_OK;
+  }
+  if (count && !dev(p)->d2h(out, p->imp_dom + first, (size_t)count * 4)) return fail(p, GSIM_ERR_CUDA, "d2h");
+  return GSIM_OK;
+}
+
+extern "C" int gsim_domain_flap_set(gsim_pool* p, const uint32_t* domains, size_t n, uint32_t period_ticks,
+                                    uint32_t bad_ppm) {
+  if (!p || (!domains && n)) return GSIM_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(p->mu);
+  if (p->sharded) return domain_sharded(p);
+  if (int rc = flap_check(p, period_ticks, bad_ppm)) return rc;
+  std::vector<uint32_t> bits;
+  if (int rc = domain_bits(p, domains, n, &bits)) return rc;
+  if (!domain_alloc(p)) return fail(p, GSIM_ERR_NOMEM, "domain column");
+  const uint32_t w = flap_word_of(period_ticks, bad_ppm);
+  for (size_t x = 0; x < n; ++x) {
+    if (domains[x] >= p->dom_tab.size()) {
+      if (w == 0u) continue;
+      p->dom_tab.resize((size_t)domains[x] + 1u, 0u);
+    }
+    p->dom_tab[domains[x]] = w;
+  }
+  if (!domain_tab_upload(p)) return fail(p, GSIM_ERR_NOMEM, "domain schedule table");
+  return GSIM_OK;
+}
+
+extern "C" int gsim_domain_flap_get(gsim_pool* p, uint32_t domain, uint32_t* period_ticks, uint32_t* bad_ppm) {
+  if (!p) return GSIM_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(p->mu);
+  if (p->sharded) return domain_sharded(p);
+  if (domain == 0u || domain > GS_DOMAIN_MAX) return fail(p, GSIM_ERR_INVALID, "domain ids are 1 .. GSIM_DOMAIN_MAX");
+  const uint32_t w = domain < p->dom_tab.size() ? p->dom_tab[domain] : 0u;
+  if (period_ticks) *period_ticks = w >> GS_FLAP_PPM_BITS;
+  if (bad_ppm) *bad_ppm = w & ((1u << GS_FLAP_PPM_BITS) - 1u);
+  return GSIM_OK;
+}
+
+extern "C" int gsim_domain_flap_bad(uint64_t seed, uint32_t domain, uint32_t period_ticks, uint32_t bad_ppm,
+                                    uint32_t tick) {
+  if (domain == 0u || domain > GS_DOMAIN_MAX) return GSIM_ERR_INVALID;
+  if (period_ticks == 0u) return 1;  // no schedule: the impairment is always in force
+  if (period_ticks > GS_FLAP_MAX_PERIOD || bad_ppm > 1000000u) return GSIM_ERR_INVALID;
+  return gs_domain_flap_bad((uint32_t)seed, (uint32_t)(seed >> 32), domain, gs_flap_word(period_ticks, bad_ppm), tick)
+             ? 1 : 0;
+}
+
+extern "C" int gsim_domain_impair(gsim_pool* p, const uint32_t* domains, size_t n, uint32_t send_loss_ppm,
+                                  uint32_t recv_loss_ppm, uint32_t delay_ticks, uint32_t flags, uint32_t* n_members) {
+  if (!p || (!domains && n)) return GSIM_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(p->mu);
+  if (p->sharded) return domain_sharded(p);
+  if (int rc = impair_check(p, send_loss_ppm, delay_ticks, recv_loss_ppm, flags)) return rc;
+  std::vector<uint32_t> bits;
+  if (int rc = domain_bits(p, domains, n, &bits)) return rc;
+  const GsImpairVal v = {ppm_to_thr(send_loss_ppm), ppm_to_thr(recv_loss_ppm), delay_ticks, flags};
+  const bool now_impaired = (v.send | v.recv | v.delay | v.flags) != 0u;
+  uint32_t counts[2] = {0, 0};
+  GsDomainOp a = {};
+  a.op = GS_DOMAIN_OP_COUNT;
+  // gsim_impair_dir_many allocates columns only for a non-empty id list: count the members first where that
+  // decides it (clearing on a pool that never was impaired, or a first directional setting)
+  if (!p->imp_loss || ((v.recv != v.send || v.flags != 0u) && !p->imp_recv)) {
+    if (int rc = domain_run(p, bits, a, counts)) return rc;
+    if (n_members) *n_members = counts[0];
+    if (!p->imp_loss && !now_impaired) return GSIM_OK;
+    if (!impair_alloc(p)) return fail(p, GSIM_ERR_NOMEM, "impairment columns");
+    if (counts[0] && (v.recv != v.send || v.flags != 0u) && !reach_alloc(p))
+      return fail(p, GSIM_ERR_NOMEM, "reachability columns");
+  }
+  a.op = GS_DOMAIN_OP_IMPAIR;
+  a.imp = {p->imp_loss, p->imp_recv, p->imp_delay, p->imp_flags};
+  a.v = v;
+  if (int rc = domain_run(p, bits, a, counts)) return rc;
+  p->n_impaired = p->n_impaired - counts[1] + (now_impaired ? counts[0] : 0u);
+  if (n_members) *n_members = counts[0];
+  impair_publish(p);
+  return GSIM_OK;
+}
+
+extern "C" int gsim_domain_crash(gsim_pool* p, const uint32_t* domains, size_t n, uint32_t* n_crashed) {
+  if (!p || (!domains && n)) return GSIM_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(p->mu);
+  if (p->sharded) return domain_sharded(p);
+  std::vector<uint32_t> bits;
+  if (int rc = domain_bits(p, domains, n, &bits)) return rc;
+  GsDomainOp a = {};
+  a.op = GS_DOMAIN_OP_CRASH;
+  a.pause_until = p->pause_cnt[0] ? p->pause_until : nullptr;  // (a resume to cancel only while somebody is paused)
+  uint32_t counts[2] = {0, 0};
+  if (int rc = domain_run(p, bits, a, counts)) return rc;
+  p->pause_cnt[0] -= counts[1];
+  if (n_crashed) *n_crashed = counts[0];
+  int rc = refresh_after_truth_change(p);
+  return rc ? fail(p, rc, "recount") : GSIM_OK;
+}
+
+extern "C" int gsim_domain_pause(gsim_pool* p, const uint32_t* domains, size_t n, uint32_t ticks, uint32_t* n_paused) {
+  if (!p || (!domains && n)) return GSIM_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(p->mu);
+  uint32_t local = 0;
+  if (!n_paused) n_paused = &local;
+  *n_paused = 0;
+  if (p->sharded) return domain_sharded(p);
+  if (int rc = pause_check(p, ticks)) return rc;
+  std::vector<uint32_t> bits;
+  if (int rc = domain_bits(p, domains, n, &bits)) return rc;
+  if (!p->imp_dom || bits.empty()) return GSIM_OK;
+  if (!pause_alloc(p)) return fail(p, GSIM_ERR_NOMEM, "pause column");
+  GsDomainOp a = {};
+  a.op = GS_DOMAIN_OP_PAUSE;
+  a.pause_until = p->pause_until;
+  a.until = p->now + ticks;
+  uint32_t counts[2] = {0, 0};
+  if (int rc = domain_run(p, bits, a, counts)) return rc;
+  return pause_done(p, a.until, counts[0], n_paused);
+}
+
+extern "C" int gsim_domain_stats_read(gsim_pool* p, uint32_t first_domain, uint32_t count, gsim_domain_stats* out) {
+  if (!p || (!out && count)) return GSIM_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(p->mu);
+  if (p->sharded) return domain_sharded(p);
+  if (first_domain == 0u || (uint64_t)first_domain + count > (uint64_t)GS_DOMAIN_MAX + 1u)
+    return fail(p, GSIM_ERR_INVALID, "the domains must lie in 1 .. GSIM_DOMAIN_MAX");
+  if (!p->imp_dom) {
+    memset(out, 0, (size_t)count * sizeof(gsim_domain_stats));
+    return GSIM_OK;
+  }
+  const GsDomainCols c = {p->d.key[p->now & 1u], p->d.meta, p->imp_dom, p->pause_until,
+                          {p->imp_loss, p->imp_recv, p->imp_delay, p->imp_flags}};
+  if (!dev(p)->domain_stats(p->d, p->g, c, p->now, first_domain, count, reinterpret_cast<GsDomainStats*>(out)))
+    return fail(p, GSIM_ERR_CUDA, "domain_stats");
   return GSIM_OK;
 }
 
@@ -3412,7 +3753,7 @@ struct SnapCol {
   bool may_fill;     // planes may be stored as a repeated word
 };
 static std::vector<SnapCol> snap_cols(gsim_pool* p, bool with_impairment, bool with_pause, bool with_reach,
-                                      bool with_flap) {
+                                      bool with_flap, bool with_dom) {
   const GsDev& d = p->d;
   const size_t cap = p->g.cap;
   std::vector<SnapCol> v;
@@ -3453,6 +3794,7 @@ static std::vector<SnapCol> snap_cols(gsim_pool* p, bool with_impairment, bool w
     add(p->pause_cnt_dev, 4 * 8, 1, false);
   }
   if (with_flap) add(p->imp_flap, cap * 4);
+  if (with_dom) add(p->imp_dom, cap * 4);  // (the schedule table follows the columns: its length, then its words)
   add(d.stats, GSIM_STAT_COUNT * 8, 1, false); add(d.heard_cnt, 32 * 4, 1, false); add(d.conv_tick, 32 * 4, 1, false);
   add(d.crashed_alive, 4, 1, false); add(d.crashed_dead_tick, 4, 1, false);
   return v;
@@ -3483,6 +3825,7 @@ static uint32_t snap_layout(const gsim_pool* p) {
   if (p->imp_recv) m |= 64u;     // the reachability columns (with bit 8; restore allocates them when the pool has none)
   if (p->d.pig) m |= 128u;       // owed answers and the piggyback words (GSIM_FLAG_PROBE_PIGGYBACK)
   if (p->imp_flap) m |= 256u;    // the flap schedule column (restore allocates it when the pool has none)
+  if (p->imp_dom) m |= 512u;     // the domain column and schedule table (restore allocates the column)
   return m;
 }
 static uint64_t snap_graph_hash(const gsim_pool* p) {
@@ -3503,8 +3846,9 @@ static size_t snap_size(gsim_pool* p) {
   size_t s = sizeof(SnapHeader) + p->sched.size() * sizeof(Sched);
   for (uint32_t r = 0; r < GS_MAX_RUMORS; ++r) s += 12 + p->rh[r].name.size() + p->rh[r].payload.size();
   for (const SnapCol& c : snap_cols(p, p->imp_loss != nullptr, p->pause_until != nullptr, p->imp_recv != nullptr,
-                                    p->imp_flap != nullptr))
+                                    p->imp_flap != nullptr, p->imp_dom != nullptr))
     s += c.bytes + 4u * c.planes;  // upper bound: every plane raw
+  if (p->imp_dom) s += 4u + p->dom_tab.size() * 4u;
   return s;
 }
 
@@ -3554,7 +3898,7 @@ extern "C" int gsim_snapshot(gsim_pool* p, void* out, size_t cap_bytes, size_t* 
   if (p->pause_cnt_dev && !dev(p)->h2d(p->pause_cnt_dev, p->pause_cnt, sizeof(p->pause_cnt)))
     return fail(p, GSIM_ERR_CUDA, "h2d");
   for (const SnapCol& c : snap_cols(p, p->imp_loss != nullptr, p->pause_until != nullptr, p->imp_recv != nullptr,
-                                    p->imp_flap != nullptr)) {
+                                    p->imp_flap != nullptr, p->imp_dom != nullptr)) {
     const size_t pb = c.bytes / c.planes;
     for (uint32_t q = 0; q < c.planes; ++q) {
       uint8_t* raw = w + 4;
@@ -3565,6 +3909,12 @@ extern "C" int gsim_snapshot(gsim_pool* p, void* out, size_t cap_bytes, size_t* 
       memcpy(w, &tag, 4);
       w += 4 + (uniform ? 4 : pb);
     }
+  }
+  if (p->imp_dom) {
+    const uint32_t len = (uint32_t)p->dom_tab.size();
+    memcpy(w, &len, 4);
+    if (len) memcpy(w + 4, p->dom_tab.data(), (size_t)len * 4);
+    w += 4 + (size_t)len * 4;
   }
   if (n_bytes) *n_bytes = (size_t)(w - w0);  // what was actually written (<= gsim_snapshot_size)
   return GSIM_OK;
@@ -3584,7 +3934,7 @@ extern "C" int gsim_restore(gsim_pool* p, const void* blob, size_t n_bytes) {
   // geometry and peer graph must be this pool's before a single plane is copied.
   if (h.cap != p->g.cap || h.g.cap != p->g.cap || h.g.n > p->cfg.capacity || h.g.n > p->g.cap ||
       h.g.ring_mask != p->g.ring_mask || (h.g.pp_interval != 0u) != (p->g.pp_interval != 0u) ||
-      (h.layout & ~360u) != (snap_layout(p) & ~360u) || (h.layout & 72u) == 64u || h.g.world != p->g.world || h.g.key_stride != p->g.key_stride ||
+      (h.layout & ~872u) != (snap_layout(p) & ~872u) || (h.layout & 72u) == 64u || h.g.world != p->g.world || h.g.key_stride != p->g.key_stride ||
       h.g.rows_per_rank != p->g.rows_per_rank || h.g.phase_group != p->g.phase_group ||
       h.g.graph_n != p->g.graph_n || h.graph_hash != snap_graph_hash(p) || h.n_established > h.g.n)
     return fail(p, GSIM_ERR_INVALID, "snapshot does not match this pool (capacity, column set, sharding or peer graph)");
@@ -3612,7 +3962,9 @@ extern "C" int gsim_restore(gsim_pool* p, const void* blob, size_t n_bytes) {
   if (blob_paused && !pause_alloc(p)) return fail(p, GSIM_ERR_NOMEM, "pause column");
   const bool blob_flap = (h.layout & 256u) != 0u;
   if (blob_flap && !flap_alloc(p)) return fail(p, GSIM_ERR_NOMEM, "schedule column");
-  for (const SnapCol& c : snap_cols(p, blob_impaired, blob_paused, blob_reach, blob_flap)) {
+  const bool blob_dom = (h.layout & 512u) != 0u;
+  if (blob_dom && !domain_alloc(p)) return fail(p, GSIM_ERR_NOMEM, "domain column");
+  for (const SnapCol& c : snap_cols(p, blob_impaired, blob_paused, blob_reach, blob_flap, blob_dom)) {
     if (c.may_fill) {  // plane by plane: a device fill or a copy
       const size_t pb = c.bytes / c.planes;
       for (uint32_t q = 0; q < c.planes; ++q) {
@@ -3659,6 +4011,19 @@ extern "C" int gsim_restore(gsim_pool* p, const void* blob, size_t n_bytes) {
   if (!blob_paused && p->pause_until && !dev(p)->fill32(p->pause_until, 0u, p->g.cap)) return fail(p, GSIM_ERR_CUDA, "fill");
   // ... and one without the schedule column a pool in which nobody has a schedule
   if (!blob_flap && p->imp_flap && !dev(p)->fill32(p->imp_flap, 0u, p->g.cap)) return fail(p, GSIM_ERR_CUDA, "fill");
+  // ... and one without domains a pool in which nobody has a domain and no domain a schedule
+  p->dom_tab.clear();
+  if (blob_dom) {
+    uint32_t len = 0;
+    if (end - r < 4) return fail(p, GSIM_ERR_INVALID, "truncated");
+    memcpy(&len, r, 4);
+    if (len > GS_DOMAIN_MAX + 1u || (size_t)(end - r - 4) < (size_t)len * 4) return fail(p, GSIM_ERR_INVALID, "truncated");
+    p->dom_tab.assign(len, 0u);
+    if (len) memcpy(p->dom_tab.data(), r + 4, (size_t)len * 4);
+    r += 4 + (size_t)len * 4;
+  } else if (p->imp_dom && !dev(p)->fill32(p->imp_dom, 0u, p->g.cap)) {
+    return fail(p, GSIM_ERR_CUDA, "fill");
+  }
   if (!dev(p)->sync()) return fail(p, GSIM_ERR_CUDA, "sync");  // every plane has left the caller's blob
   // ... and one without the reachability columns a pool whose settings are all symmetric
   if (!blob_reach && p->imp_recv) {
@@ -3684,7 +4049,7 @@ extern "C" int gsim_restore(gsim_pool* p, const void* blob, size_t n_bytes) {
   p->n_established = h.n_established;
   p->g_dirty = true;
   counts_invalidate(p);
-  if (!impair_recount(p) || !flap_recount(p)) return fail(p, GSIM_ERR_CUDA, "d2h");
+  if (!impair_recount(p) || !flap_recount(p) || !domain_tab_upload(p)) return fail(p, GSIM_ERR_CUDA, "d2h");
   if (!poke(p, p->d.tick_base, 0, p->now) || !reset_tick_flags(p) || !reset_qstate(p)) return fail(p, GSIM_ERR_CUDA, "poke");
   uint32_t zero2[2] = {0, 0};
   if (!dev(p)->h2d(p->d.evlog_cursor, zero2, 8)) return fail(p, GSIM_ERR_CUDA, "h2d");

@@ -56,6 +56,12 @@ GS_DEV void gs_init_row(const GsDev& d, const GsGlobals& g, uint32_t i, uint32_t
   }
 }
 
+// Member i (key word k0 in buffer 0) crashes: truth CRASHED in both key buffers.
+GS_DEV void gs_crash_keys(const GsDev& d, const GsGlobals& g, uint32_t i, uint32_t k0) {
+  gs_key_store(d, g, 0u, i, (k0 & ~3u) | GS_TRUTH_CRASHED);
+  gs_key_store(d, g, 1u, i, (d.key[1][i] & ~3u) | GS_TRUTH_CRASHED);
+}
+
 // BASELINE config 3: crash every UP member whose Philox draw is below the threshold.
 GS_DEV bool gs_crash_row(const GsDev& d, const GsGlobals& g, uint32_t i, uint32_t thr,
                          uint32_t salt) {
@@ -63,9 +69,7 @@ GS_DEV bool gs_crash_row(const GsDev& d, const GsGlobals& g, uint32_t i, uint32_
   if (gs_key_truth(k) != GS_TRUTH_UP) return false;
   GsU4 r = gs_philox(g.seed_lo, g.seed_hi, i, salt, GS_PUR_CRASH, 0u);
   if (r.x >= thr) return false;
-  k = (k & ~3u) | GS_TRUTH_CRASHED;
-  gs_key_store(d, g, 0u, i, k);
-  gs_key_store(d, g, 1u, i, (d.key[1][i] & ~3u) | GS_TRUTH_CRASHED);
+  gs_crash_keys(d, g, i, k);
   return true;
 }
 
@@ -119,6 +123,67 @@ GS_DEV uint32_t gs_resume_row(const GsDev& d, const GsGlobals& g, uint32_t* paus
   }
   pause_until[i] = 0u;
   return GS_PAUSE_FORGOTTEN;
+}
+
+// ---- fault domains (gsim_domain_*, DESIGN.md §3.5 "Fault domains") -----------------------------------
+// dom = the domain column; bits = a bitmap of the listed domains (domain x is bit x & 31 of word x >> 5,
+// n_words words).  The one selection rule of gsim_domain_impair, _crash and _pause: member i's domain is listed.
+GS_HD bool gs_domain_listed(const uint32_t* dom, const uint32_t* bits, uint32_t n_words, uint32_t i) {
+  const uint32_t x = dom[i];
+  return x != 0u && (x >> 5) < n_words && ((bits[x >> 5] >> (x & 31u)) & 1u) != 0u;
+}
+
+// One listed member of a domain operation, as the per-member call would treat it.  Returns bit 0 = counted in
+// counts[0] (IMPAIR: written; CRASH: crashed; PAUSE: paused), bit 1 = counted in counts[1] (IMPAIR: it was
+// impaired before; CRASH: a paused member whose resume was cancelled).  COUNT writes nothing and counts it.
+GS_DEV uint32_t gs_domain_op_row(const GsDev& d, const GsGlobals& g, const GsDomainOp& a, uint32_t i) {
+  if (a.op == GS_DOMAIN_OP_COUNT) return 1u;
+  if (a.op == GS_DOMAIN_OP_IMPAIR) return gs_impair_write(a.imp, i, a.v) ? 3u : 1u;  // gsim_impair_dir_many
+  if (a.op == GS_DOMAIN_OP_PAUSE) return gs_pause_row(d, g, a.pause_until, i, a.until) ? 1u : 0u;
+  const uint32_t k = d.key[0][i];  // gsim_crash_many: a running member crashes, a paused one crashes for good
+  if (gs_key_truth(k) == GS_TRUTH_UP) {
+    gs_crash_keys(d, g, i, k);
+    return 1u;
+  }
+  if (gs_key_truth(k) == GS_TRUTH_CRASHED && a.pause_until != nullptr && a.pause_until[i] != 0u) {
+    a.pause_until[i] = 0u;
+    return 2u;
+  }
+  return 0u;
+}
+
+// Member i's contribution to its domain's stats at tick now, packed as the stats kernel sums them: c[0] =
+// members | running << 6 | paused << 12 | impaired << 18 | in_force << 24, c[1] = alive | suspect << 6 | dead
+// << 12 | left << 18, c[2] = its awareness when it runs (else 0).  Returns false when it is not counted (truth
+// NONE).
+GS_HD bool gs_domain_stats_row(const GsDev& d, uint32_t seed_lo, uint32_t seed_hi, const GsDomainCols& c, uint32_t i,
+                               uint32_t now, uint32_t out[3]) {
+  const uint32_t k = c.key[i];
+  if (gs_key_truth(k) == GS_TRUTH_NONE) return false;
+  const bool run = gs_key_truth(k) == GS_TRUTH_UP;
+  const bool paused = c.pause_until != nullptr && c.pause_until[i] != 0u;
+  const GsImpairCols& m = c.imp;
+  const bool impaired = (m.loss != nullptr && m.loss[i] != 0u) || (m.recv != nullptr && m.recv[i] != 0u) ||
+                        (m.delay != nullptr && m.delay[i] != 0u) || (m.flags != nullptr && m.flags[i] != 0u);
+  const bool in_force = impaired && gs_imp_in_force(d, seed_lo, seed_hi, i, now);
+  out[0] = 1u | (run ? 1u << 6 : 0u) | (paused ? 1u << 12 : 0u) | (impaired ? 1u << 18 : 0u) |
+           (in_force ? 1u << 24 : 0u);
+  out[1] = 1u << (6u * gs_key_rank(k));
+  out[2] = run ? gs_meta_aw(c.meta[i]) : 0u;
+  return true;
+}
+GS_HD void gs_domain_stats_add(GsDomainStats& s, const uint32_t c[3], uint32_t aw_max) {
+  s.members += c[0] & 63u;
+  s.running += (c[0] >> 6) & 63u;
+  s.paused += (c[0] >> 12) & 63u;
+  s.impaired += (c[0] >> 18) & 63u;
+  s.in_force += (c[0] >> 24) & 63u;
+  s.alive += c[1] & 63u;
+  s.suspect += (c[1] >> 6) & 63u;
+  s.dead += (c[1] >> 12) & 63u;
+  s.left += (c[1] >> 18) & 63u;
+  s.awareness_sum += c[2];
+  if (aw_max > s.awareness_max) s.awareness_max = aw_max;
 }
 
 // [U] serf.handleReap -> reap(failedMembers, ReconnectTimeout) / reap(leftMembers, TombstoneTimeout):

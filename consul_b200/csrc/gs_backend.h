@@ -278,6 +278,17 @@ class GsBackend {
                           uint32_t* n_paused);
   virtual bool resume_rows(const GsDev& d, const GsGlobals* g_dev, const GsGlobals& g, uint32_t* pause_until,
                            uint32_t t, bool resume, bool log_events, uint32_t counts[4]);
+  // Fault domains (gs_aux.h; dom is the caller's domain column).  domain_range: dom[first + x] = first_domain +
+  // x / per_domain for x < count.  domain_rows: gs_domain_op_row(a) over every member gs_domain_listed selects,
+  // `bits` a host bitmap of n_words words; counts[0] and counts[1] sum its two result bits.  domain_stats: out[x]
+  // (host memory) = the stats of domain first_domain + x at tick now, gs_domain_stats_row summed over its
+  // members.  Defined in gs_api.cpp through the copy primitives every backend has, which is what the host
+  // emulation runs; the CUDA backend replaces each with one sm_90a kernel.
+  virtual bool domain_range(uint32_t* dom, uint32_t first, uint32_t count, uint32_t per_domain, uint32_t first_domain);
+  virtual bool domain_rows(const GsDev& d, const GsGlobals* g_dev, const GsGlobals& g, const uint32_t* dom,
+                           const uint32_t* bits, uint32_t n_words, const GsDomainOp& a, uint32_t counts[2]);
+  virtual bool domain_stats(const GsDev& d, const GsGlobals& g, const GsDomainCols& c, uint32_t now,
+                            uint32_t first_domain, uint32_t count, GsDomainStats* out);
   // ---- network-coordinate queries (gs_query.h, DESIGN.md §3.4 "Queries"; single-GPU pools) ----------
   // Read-only.  Every pointer is device memory and nothing is waited for: the caller reads the result
   // back once.  Defined in gs_api.cpp through the copy primitives every backend has, which is what the

@@ -66,7 +66,8 @@ enum {
   GS_PUR_IMPAIR = 9,
   GS_PUR_PAUSE = 10,
   // 11 = gsim_coordinate_error's sample draws (GS_PUR_COORD_SAMPLE)
-  GS_PUR_FLAP = 12
+  GS_PUR_FLAP = 12,
+  GS_PUR_FLAP_DOMAIN = 13
 };
 // Loss "kind" (folded into the counter) — one draw per simulated UDP packet.
 enum {
@@ -306,18 +307,22 @@ struct GsImpairVal {
 // gsim_impair_fraction / gsim_impair_dir_fraction for member i whose key word (either buffer: truth is in
 // both) is key: a member that runs and whose Philox draw (its own purpose word, so the selection is
 // independent of gs_crash_row's for the same salt) is below thr gets the impairment v (recv and flags only
-// where those columns exist).  Returns bit 0 = selected, bit 1 = it was impaired before.
-GS_HD uint32_t gs_impair_row(uint32_t key, const GsImpairCols& c, uint32_t seed_lo, uint32_t seed_hi, uint32_t i,
-                             uint32_t thr, uint32_t salt, const GsImpairVal& v) {
-  if ((key & 3u) != GS_TRUTH_UP) return 0u;
-  if (gs_philox(seed_lo, seed_hi, i, salt, GS_PUR_IMPAIR, 0u).x >= thr) return 0u;
+// where those columns exist, gs_impair_write: returns whether member i was impaired before).  Returns bit 0 =
+// selected, bit 1 = it was impaired before.
+GS_HD bool gs_impair_write(const GsImpairCols& c, uint32_t i, const GsImpairVal& v) {
   const bool was = c.loss[i] != 0u || c.delay[i] != 0u || (c.recv != nullptr && c.recv[i] != 0u) ||
                    (c.flags != nullptr && c.flags[i] != 0u);
   c.loss[i] = v.send;
   c.delay[i] = (uint8_t)v.delay;
   if (c.recv != nullptr) c.recv[i] = v.recv;
   if (c.flags != nullptr) c.flags[i] = (uint8_t)v.flags;
-  return was ? 3u : 1u;
+  return was;
+}
+GS_HD uint32_t gs_impair_row(uint32_t key, const GsImpairCols& c, uint32_t seed_lo, uint32_t seed_hi, uint32_t i,
+                             uint32_t thr, uint32_t salt, const GsImpairVal& v) {
+  if ((key & 3u) != GS_TRUTH_UP) return 0u;
+  if (gs_philox(seed_lo, seed_hi, i, salt, GS_PUR_IMPAIR, 0u).x >= thr) return 0u;
+  return gs_impair_write(c, i, v) ? 3u : 1u;
 }
 
 // Intermittent impairment (gsim_impair_flap_*): a member's schedule word is period << 20 | bad_ppm, 0 for
@@ -327,19 +332,41 @@ GS_HD uint32_t gs_impair_row(uint32_t key, const GsImpairCols& c, uint32_t seed_
 #define GS_FLAP_MAX_PERIOD 4095u
 GS_HD uint32_t gs_flap_word(uint32_t period, uint32_t bad_ppm) { return period << GS_FLAP_PPM_BITS | bad_ppm; }
 
-// Is member m in a bad epoch at tick t under schedule word w (w != 0)?  phase = philox(m, ~0, FLAP).y mod
-// period; epoch = (t + phase) / period in 64 bits; bad iff philox(m, epoch, FLAP).x < thr(bad_ppm), the ppm
-// threshold floor(ppm 2^32 / 1e6), except that 1e6 is bad in every epoch.
-GS_HD bool gs_flap_bad(uint32_t seed_lo, uint32_t seed_hi, uint32_t m, uint32_t w, uint32_t t) {
+// Is the epoch of tick t bad under schedule word w (w != 0) for key k drawn under purpose word pur?  phase =
+// philox(k, ~0, pur).y mod period; epoch = (t + phase) / period in 64 bits; bad iff philox(k, epoch, pur).x <
+// thr(bad_ppm), the ppm threshold floor(ppm 2^32 / 1e6), except that 1e6 is bad in every epoch.  Members
+// (gs_flap_bad) and fault domains (gs_domain_flap_bad) draw their epochs here, each under its own purpose word.
+GS_HD bool gs_epoch_bad(uint32_t seed_lo, uint32_t seed_hi, uint32_t k, uint32_t pur, uint32_t w, uint32_t t) {
   const uint32_t period = w >> GS_FLAP_PPM_BITS, ppm = w & ((1u << GS_FLAP_PPM_BITS) - 1u);
   if (ppm >= 1000000u) return true;
   if (ppm == 0u) return false;
-  const uint32_t phase = gs_philox(seed_lo, seed_hi, m, 0xFFFFFFFFu, GS_PUR_FLAP, 0u).y % period;
+  const uint32_t phase = gs_philox(seed_lo, seed_hi, k, 0xFFFFFFFFu, pur, 0u).y % period;
   // (t + phase) / period without a 64-bit division: t = q period + r, and r + phase < 2 period
   const uint32_t q = t / period, r = t - q * period;
   const uint32_t epoch = q + (r + phase >= period ? 1u : 0u);
   const uint32_t thr = (uint32_t)(((uint64_t)ppm << 32) / 1000000u);
-  return gs_philox(seed_lo, seed_hi, m, epoch, GS_PUR_FLAP, 0u).x < thr;
+  return gs_philox(seed_lo, seed_hi, k, epoch, pur, 0u).x < thr;
+}
+
+// Is member m in a bad epoch of its own schedule w at tick t?
+GS_HD bool gs_flap_bad(uint32_t seed_lo, uint32_t seed_hi, uint32_t m, uint32_t w, uint32_t t) {
+  return gs_epoch_bad(seed_lo, seed_hi, m, GS_PUR_FLAP, w, t);
+}
+
+// Fault domains (gsim_domain_*): each member has a domain id (0 = none, 1 .. GS_DOMAIN_MAX), and a domain may
+// have a schedule word of the same format as a member's.  Is domain dom in a bad epoch of w at tick t?
+#define GS_DOMAIN_MAX ((1u << 22) - 1u)
+GS_HD bool gs_domain_flap_bad(uint32_t seed_lo, uint32_t seed_hi, uint32_t dom, uint32_t w, uint32_t t) {
+  return gs_epoch_bad(seed_lo, seed_hi, dom, GS_PUR_FLAP_DOMAIN, w, t);
+}
+
+// The two layers of intermittent impairment: member m's impairment is in force at t iff its own schedule wm
+// is absent (0) or bad at t, and its domain's schedule wd is absent (0: no domain, or a domain without one)
+// or bad at t.
+GS_HD bool gs_in_force(uint32_t seed_lo, uint32_t seed_hi, uint32_t m, uint32_t wm, uint32_t dom, uint32_t wd,
+                       uint32_t t) {
+  return (wm == 0u || gs_flap_bad(seed_lo, seed_hi, m, wm, t)) &&
+         (wd == 0u || gs_domain_flap_bad(seed_lo, seed_hi, dom, wd, t));
 }
 
 // gsim_impair_flap_fraction for member i: the selection of gs_impair_row (same draw, so a salt picks the
@@ -517,7 +544,54 @@ struct GsDev {
   // schedule or nobody is impaired.  Only the impaired row step reads it; last in the struct, so every other
   // field keeps its offset.
   const uint32_t* imp_flap;
+  // fault domains (gsim_domain_*): the domain column and the domain schedule table (dom_flap[x] = schedule
+  // word of domain x, dom_flap_n entries), both null while no domain has a schedule or nobody is impaired
+  const uint32_t* imp_dom;
+  const uint32_t* dom_flap;
+  uint32_t dom_flap_n;
 };
+
+// Fault-domain operations and observation (bodies in gs_aux.h).
+enum { GS_DOMAIN_OP_IMPAIR = 0, GS_DOMAIN_OP_CRASH = 1, GS_DOMAIN_OP_PAUSE = 2, GS_DOMAIN_OP_COUNT = 3 };
+// What a domain operation writes: the impairment columns and setting (IMPAIR), the pause column (CRASH: null
+// while nobody was ever paused; PAUSE) and the resume tick (PAUSE).
+struct GsDomainOp {
+  uint32_t op;
+  GsImpairCols imp;
+  GsImpairVal v;
+  uint32_t* pause_until;
+  uint32_t until;
+};
+
+// Per-domain observation (gsim_domain_stats_read), field for field gsim_domain_stats.
+struct GsDomainStats {
+  uint32_t members, running, paused, impaired, in_force;
+  uint32_t alive, suspect, dead, left;
+  uint32_t awareness_max;
+  uint64_t awareness_sum;
+};
+// The columns it reads: key = the key buffer of the current tick; imp = the impairment columns (any may be
+// null); pause_until may be null; d = the published columns gs_imp_in_force reads.
+struct GsDomainCols {
+  const uint32_t* key;
+  const uint32_t* meta;
+  const uint32_t* dom;
+  const uint32_t* pause_until;
+  GsImpairCols imp;
+};
+// Member m's domain schedule word under the published columns of d (0 without one).
+GS_HD uint32_t gs_dom_word(const GsDev& d, uint32_t m, uint32_t* dom) {
+  if (d.dom_flap == nullptr) return 0u;
+  *dom = d.imp_dom[m];
+  return *dom < d.dom_flap_n ? d.dom_flap[*dom] : 0u;
+}
+
+// Is member m's impairment in force at tick t under the published columns of d (gs_in_force)?
+GS_HD bool gs_imp_in_force(const GsDev& d, uint32_t seed_lo, uint32_t seed_hi, uint32_t m, uint32_t t) {
+  uint32_t dom = 0u;
+  const uint32_t wm = d.imp_flap != nullptr ? d.imp_flap[m] : 0u, wd = gs_dom_word(d, m, &dom);
+  return gs_in_force(seed_lo, seed_hi, m, wm, dom, wd, t);
+}
 
 // Broadcasts piggybacked on probe traffic (GSIM_FLAG_PROBE_PIGGYBACK, DESIGN.md §3.7).
 #define GS_PIGK 4u       // owed answers one member serves per tick (smallest entries win), like GS_PPK

@@ -199,7 +199,7 @@ __device__ __noinline__ void gs_row_step_call(const GsDev* dp, const GsGlobals* 
   gs_row_step_body<false>(*dp, *gp, i, t, t % gp->GI, inb, sink);
 }
 
-// Pools whose impaired members have flap schedules (GsDev::imp_flap set, only with imp_loss) likewise; only
+// Pools whose impaired members have flap schedules (GsDev::imp_flap or dom_flap set, only with imp_loss) likewise; only
 // the COORDS kernels call it (gs_kernel_extras).
 template <bool COORDS, bool PIG>
 __device__ __noinline__ void gs_row_step_flap_call(const GsDev* dp, const GsGlobals* gp, uint32_t i, uint32_t t,
@@ -214,7 +214,7 @@ template <bool COORDS>
 __device__ __forceinline__ void gs_row_step_any(const GsDev* dp, const GsGlobals* gp, uint32_t i, uint32_t t,
                                                 uint32_t inb, uint32_t* s_stat, uint32_t* s_heard, uint32_t* s_q) {
   if constexpr (COORDS) {
-    if (dp->imp_flap != nullptr) {
+    if (dp->imp_flap != nullptr || dp->dom_flap != nullptr) {
       if (dp->pig == nullptr) gs_row_step_flap_call<COORDS, false>(dp, gp, i, t, inb, s_stat, s_heard, s_q);
       else gs_row_step_flap_call<COORDS, true>(dp, gp, i, t, inb, s_stat, s_heard, s_q);
       return;
@@ -1102,6 +1102,65 @@ __global__ void __launch_bounds__(GS_BLOCK)
   if (threadIdx.x < 2u && s[threadIdx.x]) atomicAdd(&out[threadIdx.x], (unsigned long long)s[threadIdx.x]);
 }
 
+// gsim_domain_set_range: dom[first + x] = first_domain + x / per_domain.
+__global__ void __launch_bounds__(GS_BLOCK)
+    gs_domain_range_kernel(uint32_t* dom, uint32_t first, uint32_t count, uint32_t per_domain, uint32_t first_domain) {
+  const uint32_t x = blockIdx.x * GS_BLOCK + threadIdx.x;
+  if (x < count) dom[first + x] = first_domain + x / per_domain;
+}
+
+// gsim_domain_impair / _crash / _pause: gs_domain_op_row for member i when its domain is listed; counts[0] and
+// counts[1] += the two result bits, aggregated per warp.
+__global__ void __launch_bounds__(GS_BLOCK)
+    gs_domain_op_kernel(GsDev d, const GsGlobals* __restrict__ gp, const uint32_t* __restrict__ dom,
+                        const uint32_t* __restrict__ bits, uint32_t n_words, GsDomainOp a, uint32_t* counts) {
+  const uint32_t i = blockIdx.x * GS_BLOCK + threadIdx.x;
+  uint32_t r = 0u;
+  if (i < gp->n && gs_domain_listed(dom, bits, n_words, i)) r = gs_domain_op_row(d, *gp, a, i);
+  const unsigned c0 = __ballot_sync(0xFFFFFFFFu, r & 1u), c1 = __ballot_sync(0xFFFFFFFFu, r & 2u);
+  if ((threadIdx.x & 31u) == 0u) {
+    if (c0) atomicAdd(&counts[0], (uint32_t)__popc(c0));
+    if (c1) atomicAdd(&counts[1], (uint32_t)__popc(c1));
+  }
+}
+
+// gsim_domain_stats_read: out[dom[i] - first_domain] += gs_domain_stats_row of member i, grid-stride.  Lanes
+// whose members share a domain (the usual case: gsim_domain_set_range gives neighbours one domain) are summed
+// in the warp first (__match_any_sync, then one reduction per packed word), so each domain a warp touches
+// takes one set of atomics.
+__global__ void __launch_bounds__(GS_BLOCK)
+    gs_domain_stats_kernel(GsDev d, GsDomainCols c, uint32_t n, uint32_t seed_lo, uint32_t seed_hi, uint32_t now,
+                           uint32_t first_domain, uint32_t count, GsDomainStats* out) {
+  const uint32_t lane = threadIdx.x & 31u;
+  for (size_t i0 = (size_t)blockIdx.x * GS_BLOCK; i0 < n; i0 += (size_t)gridDim.x * GS_BLOCK) {
+    const uint32_t i = (uint32_t)(i0 + threadIdx.x);
+    uint32_t v[3] = {0u, 0u, 0u}, x = 0xFFFFFFFFu;
+    bool on = false;
+    if (i < n) {
+      x = c.dom[i] - first_domain;
+      on = x < count && gs_domain_stats_row(d, seed_lo, seed_hi, c, i, now, v);
+    }
+    const unsigned act = __ballot_sync(0xFFFFFFFFu, on);
+    if (!on) continue;
+    const unsigned peers = __match_any_sync(act, x);
+    const uint32_t s0 = __reduce_add_sync(peers, v[0]), s1 = __reduce_add_sync(peers, v[1]);
+    const uint32_t s2 = __reduce_add_sync(peers, v[2]), mx = __reduce_max_sync(peers, v[2]);
+    if (lane != (uint32_t)__ffs(peers) - 1u) continue;
+    GsDomainStats& o = out[x];
+    atomicAdd(&o.members, s0 & 63u);
+    if ((s0 >> 6) & 63u) atomicAdd(&o.running, (s0 >> 6) & 63u);
+    if ((s0 >> 12) & 63u) atomicAdd(&o.paused, (s0 >> 12) & 63u);
+    if ((s0 >> 18) & 63u) atomicAdd(&o.impaired, (s0 >> 18) & 63u);
+    if ((s0 >> 24) & 63u) atomicAdd(&o.in_force, (s0 >> 24) & 63u);
+    if (s1 & 63u) atomicAdd(&o.alive, s1 & 63u);
+    if ((s1 >> 6) & 63u) atomicAdd(&o.suspect, (s1 >> 6) & 63u);
+    if ((s1 >> 12) & 63u) atomicAdd(&o.dead, (s1 >> 12) & 63u);
+    if ((s1 >> 18) & 63u) atomicAdd(&o.left, (s1 >> 18) & 63u);
+    if (mx) atomicMax(&o.awareness_max, mx);
+    if (s2) atomicAdd(reinterpret_cast<unsigned long long*>(&o.awareness_sum), (unsigned long long)s2);
+  }
+}
+
 // gsim_pause_many (ids != nullptr: thread x takes member ids[x], no id twice) and gsim_pause_fraction (thread i
 // takes member i): gs_pause_row, *n_paused += members paused.
 __global__ void __launch_bounds__(GS_BLOCK)
@@ -1262,8 +1321,10 @@ __global__ void __launch_bounds__(GS_BLOCK)
   if (threadIdx.x < GS_HIST_BINS && s[threadIdx.x]) atomicAdd(&out[threadIdx.x], (unsigned long long)s[threadIdx.x]);
 }
 
-// The tick and window kernels with COORDS = true: pools with network coordinates or flap schedules.
-static bool gs_kernel_extras(const GsDev& d) { return d.coord != nullptr || d.imp_flap != nullptr; }
+// The tick and window kernels with COORDS = true: pools with network coordinates or flap schedules (member or domain).
+static bool gs_kernel_extras(const GsDev& d) {
+  return d.coord != nullptr || d.imp_flap != nullptr || d.dom_flap != nullptr;
+}
 
 // Tick launches use programmatic stream serialization (PDL) so consecutive ticks overlap
 // launch latency and prologue with the previous tick's tail.
@@ -1369,7 +1430,7 @@ __global__ void __launch_bounds__(GS_BLOCK)
   gs_coord_pick(d.coord, d.ctag, g.cap, i, ci);
   gs_coord_pick(d.coord, d.ctag, g.cap, j, cj);
   est[k] = gs_coord_distance_seconds(ci, cj);
-  if (tru != nullptr) tru[k] = gs_model_rtt(g, d.imp_delay, d.imp_flap, i, j, now);
+  if (tru != nullptr) tru[k] = gs_model_rtt(g, d, i, j, now);
 }
 
 __global__ void __launch_bounds__(GS_BLOCK)
@@ -2004,6 +2065,53 @@ class CudaBackend : public GsBackend {
     const bool launched = ok(cudaGetLastError(), "pause launch");
     if (dids) cudaFreeAsync(dids, stream_);
     return launched && d2h(n_paused, cnt, 4);
+  }
+  bool domain_range(uint32_t* dom, uint32_t first, uint32_t count, uint32_t per_domain, uint32_t first_domain) override {
+    cudaSetDevice(dev_);
+    if (!count) return true;
+    gs_domain_range_kernel<<<(count + GS_BLOCK - 1) / GS_BLOCK, GS_BLOCK, 0, stream_>>>(dom, first, count, per_domain,
+                                                                                       first_domain);
+    ++launches_;
+    return ok(cudaGetLastError(), "domain range launch");
+  }
+  bool domain_rows(const GsDev& d, const GsGlobals* g_dev, const GsGlobals& g, const uint32_t* dom, const uint32_t* bits,
+                   uint32_t n_words, const GsDomainOp& a, uint32_t counts[2]) override {
+    cudaSetDevice(dev_);
+    uint32_t* cnt = reinterpret_cast<uint32_t*>(scratch_);
+    if (!ok(cudaMemsetAsync(cnt, 0, 8, stream_), "memset")) return false;
+    uint32_t* dbits = nullptr;
+    if (g.n && n_words) {  // the bitmap travels with the launch (pageable source: copied before the call returns)
+      if (!ok(cudaMallocAsync(reinterpret_cast<void**>(&dbits), (size_t)n_words * 4, stream_), "malloc")) return false;
+      if (!ok(cudaMemcpyAsync(dbits, bits, (size_t)n_words * 4, cudaMemcpyHostToDevice, stream_), "h2d")) {
+        cudaFreeAsync(dbits, stream_);
+        return false;
+      }
+      gs_domain_op_kernel<<<(g.n + GS_BLOCK - 1) / GS_BLOCK, GS_BLOCK, 0, stream_>>>(d, g_dev, dom, dbits, n_words, a,
+                                                                                     cnt);
+      ++launches_;
+    }
+    const bool launched = ok(cudaGetLastError(), "domain launch");
+    if (dbits) cudaFreeAsync(dbits, stream_);
+    return launched && d2h(counts, cnt, 8);
+  }
+  bool domain_stats(const GsDev& d, const GsGlobals& g, const GsDomainCols& c, uint32_t now, uint32_t first_domain,
+                    uint32_t count, GsDomainStats* out) override {
+    cudaSetDevice(dev_);
+    if (!count) return true;
+    const size_t bytes = (size_t)count * sizeof(GsDomainStats);
+    GsDomainStats* dout = nullptr;
+    if (!ok(cudaMallocAsync(reinterpret_cast<void**>(&dout), bytes, stream_), "malloc")) return false;
+    bool okk = ok(cudaMemsetAsync(dout, 0, bytes, stream_), "memset");
+    if (okk && g.n) {
+      const uint32_t blocks = (g.n + GS_BLOCK - 1) / GS_BLOCK < sms_ * 8u ? (g.n + GS_BLOCK - 1) / GS_BLOCK : sms_ * 8u;
+      gs_domain_stats_kernel<<<blocks, GS_BLOCK, 0, stream_>>>(d, c, g.n, g.seed_lo, g.seed_hi, now, first_domain, count,
+                                                               dout);
+      ++launches_;
+      okk = ok(cudaGetLastError(), "domain stats launch");
+    }
+    okk = okk && d2h(out, dout, bytes);
+    cudaFreeAsync(dout, stream_);
+    return okk;
   }
   bool resume_rows(const GsDev& d, const GsGlobals* g_dev, const GsGlobals& g, uint32_t* pause_until, uint32_t t,
                    bool resume, bool log_events, uint32_t counts[4]) override {

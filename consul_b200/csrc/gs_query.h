@@ -21,13 +21,32 @@ GS_DEV void gs_coord_pick(const double* coord, const uint32_t* ctag, size_t cap,
   c.height = base[(size_t)10 * cap];
 }
 
-// The round trip a direct probe between a and b would sample at tick `now` (gs_coord_on_ack): the latency
-// matrix and the receivers' delays there and back.  `delay` = GsDev::imp_delay (null while nobody is
-// impaired), `flap` = GsDev::imp_flap (a scheduled receiver's delay counts only in its bad epochs).
-GS_DEV double gs_model_rtt(const GsGlobals& g, const uint8_t* delay, const uint32_t* flap, uint32_t a, uint32_t b,
-                           uint32_t now) {
-  return g.coord_base_rtt_s + (double)(gs_extra(g, delay, a, b, gs_imp_on(g, flap, b, now)) +
-                                       gs_extra(g, delay, b, a, gs_imp_on(g, flap, a, now))) *
+// Is member m's impairment in force at tick `now` (gs_imp_in_force), for pools with member or domain
+// schedules only: out of line, so that the query kernels of pools without schedules do not carry the
+// schedule lookups (column pointers by value: taking the address of the kernel's GsDev parameter would copy
+// it to the stack).
+#if defined(__CUDA_ARCH__)
+__device__ __noinline__
+#else
+inline
+#endif
+uint32_t gs_rtt_on(uint32_t seed_lo, uint32_t seed_hi, const uint32_t* flap, const uint32_t* dom,
+                   const uint32_t* dom_flap, uint32_t dom_flap_n, uint32_t m, uint32_t now) {
+  const uint32_t wm = flap != nullptr ? flap[m] : 0u;
+  const uint32_t x = dom_flap != nullptr ? dom[m] : 0u, wd = x != 0u && x < dom_flap_n ? dom_flap[x] : 0u;
+  return gs_in_force(seed_lo, seed_hi, m, wm, x, wd, now) ? 1u : 0u;
+}
+
+// The round trip a direct probe between a and b would sample at tick `now` (gs_coord_on_ack): the latency matrix and
+// the receivers' delays there and back, each while that receiver's impairment is in force (d.imp_delay is null
+// while nobody is impaired; without member or domain schedules every impairment is in force).
+GS_DEV double gs_model_rtt(const GsGlobals& g, const GsDev& d, uint32_t a, uint32_t b, uint32_t now) {
+  uint32_t on_a = 1u, on_b = 1u;
+  if (d.imp_flap != nullptr || d.dom_flap != nullptr) {
+    on_a = gs_rtt_on(g.seed_lo, g.seed_hi, d.imp_flap, d.imp_dom, d.dom_flap, d.dom_flap_n, a, now);
+    on_b = gs_rtt_on(g.seed_lo, g.seed_hi, d.imp_flap, d.imp_dom, d.dom_flap, d.dom_flap_n, b, now);
+  }
+  return g.coord_base_rtt_s + (double)(gs_extra(g, d.imp_delay, a, b, on_b) + gs_extra(g, d.imp_delay, b, a, on_a)) *
                                   g.tick_seconds;
 }
 
@@ -80,7 +99,7 @@ GS_DEV double gs_error_draw(const GsDev& d, const GsGlobals& g, uint32_t now, ui
   GsCoord a, b;
   gs_coord_pick(d.coord, d.ctag, g.cap, i, a);
   gs_coord_pick(d.coord, d.ctag, g.cap, j, b);
-  const double est = gs_coord_distance_seconds(a, b), tru = gs_model_rtt(g, d.imp_delay, d.imp_flap, i, j, now);
+  const double est = gs_coord_distance_seconds(a, b), tru = gs_model_rtt(g, d, i, j, now);
   return fabs(est - tru) / tru;
 }
 

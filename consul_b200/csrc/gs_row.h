@@ -201,15 +201,14 @@ GS_DEV GsHot gs_hot(const GsGlobals& g) {
   return h;
 }
 
-// Is member m's impairment in force at tick t (1) or not (0)?  `flap` = GsDev::imp_flap (schedule words, null
-// while no member has one): a member without a schedule is always impaired, one with a schedule only in its
-// bad epochs (gs_flap_bad).  The row step asks once per member it deals with and hands the answers to the
-// helpers below as `on` bits: bit 0 for the packet's sender (or member i), bit 1 for its receiver (or j).
+// Is member m's impairment in force at tick t (1) or not (0)?  Both layers of schedules (gs_imp_in_force over
+// GsDev::imp_flap and the fault-domain columns imp_dom / dom_flap, each null while unused): a member in force
+// is one whose own schedule and whose domain's schedule are each absent or bad at t.  The row step asks once
+// per member it deals with and hands the answers to the helpers below as `on` bits: bit 0 for the packet's
+// sender (or member i), bit 1 for its receiver (or j).
 template <class G>
-GS_DEV uint32_t gs_imp_on(const G& g, const uint32_t* flap, uint32_t m, uint32_t t) {
-  if (flap == nullptr) return 1u;
-  const uint32_t w = flap[m];
-  return w == 0u || gs_flap_bad(g.seed_lo, g.seed_hi, m, w, t) ? 1u : 0u;
+GS_DEV uint32_t gs_imp_on(const G& g, const GsDev& d, uint32_t m, uint32_t t) {
+  return gs_imp_in_force(d, g.seed_lo, g.seed_hi, m, t) ? 1u : 0u;
 }
 
 // `delay` = the receive-delay column of a pool with impaired members (GsDev::imp_delay), else null:
@@ -580,15 +579,15 @@ GS_DEV bool gs_mail_is_stale(const GsGlobals& g, uint32_t w, uint32_t heard, boo
 // away, so a pool without any runs the code it would run without the feature.
 // PIG: the pool piggybacks broadcasts on probe traffic (GsDev::pig_req / pig are set); likewise folded away
 // in the other instantiation.
-// FLAP (with IMPAIRED): some impaired member has a flap schedule (GsDev::imp_flap is set); the impaired
-// instantiation without it folds every schedule term away, so impaired pools without schedules run the code
-// they ran before the feature.
+// FLAP (with IMPAIRED): some impaired member has a flap schedule, or some fault domain has one (GsDev::imp_flap
+// or dom_flap is set); the impaired instantiation without it folds every schedule term away, so impaired pools
+// without schedules run the code they ran before the feature.
 // FLAP: whether member x's impairment is in force at t (gs_imp_on); the row step asks once per member and stage
 // where it is needed, keeping the answers out of long live ranges (it runs at the register limit).  Every other
 // instantiation folds the `on` bits to 1.
 template <bool FLAP>
 GS_DEV uint32_t gs_on(const GsDev& d, const GsGlobals& g, uint32_t x, uint32_t t) {
-  return FLAP ? gs_imp_on(g, d.imp_flap, x, t) : 1u;
+  return FLAP ? gs_imp_on(g, d, x, t) : 1u;
 }
 
 template <bool IMPAIRED, bool PIG = false, bool FLAP = false, class Sink>
@@ -870,7 +869,7 @@ GS_DEV void gs_row_step_body(const GsDev& d, const GsGlobals& g, uint32_t i, uin
       // a direct ack that was merely slower than ProbeTimeout still counts until the deadline (its loss draws
       // are the probe's, at t0, and so are the ends' schedules)
       if ((g.n_dcs != 0u || imp_delay != nullptr) && j_up && rtt_ij > g.T && rtt_ij <= budget + g.T) {
-        const uint32_t on0 = FLAP ? gs_imp_on(g, d.imp_flap, i, t0) | gs_imp_on(g, d.imp_flap, j, t0) << 1 : 3u;
+        const uint32_t on0 = FLAP ? gs_imp_on(g, d, i, t0) | gs_imp_on(g, d, j, t0) << 1 : 3u;
         if (!gs_lost_quiet(g, imp_loss, i, j, t0, GS_LK_PING, 0, on0) &&
             !gs_lost_quiet(g, imp_loss, j, i, t0, GS_LK_ACK, 0, on0 >> 1 | (on0 & 1u) << 1))
           success = true;
@@ -1128,12 +1127,12 @@ template <class Sink>
 GS_DEV void gs_row_step(const GsDev& d, const GsGlobals& g, uint32_t i, uint32_t t, uint32_t gslot, uint32_t inb,
                         Sink& sink) {
   if (d.pig != nullptr) {
-    if (d.imp_flap != nullptr) gs_row_step_body<true, true, true>(d, g, i, t, gslot, inb, sink);
+    if (d.imp_flap != nullptr || d.dom_flap != nullptr) gs_row_step_body<true, true, true>(d, g, i, t, gslot, inb, sink);
     else if (d.imp_loss != nullptr) gs_row_step_body<true, true>(d, g, i, t, gslot, inb, sink);
     else gs_row_step_body<false, true>(d, g, i, t, gslot, inb, sink);
     return;
   }
-  if (d.imp_flap != nullptr) gs_row_step_body<true, false, true>(d, g, i, t, gslot, inb, sink);
+  if (d.imp_flap != nullptr || d.dom_flap != nullptr) gs_row_step_body<true, false, true>(d, g, i, t, gslot, inb, sink);
   else if (d.imp_loss != nullptr) gs_row_step_body<true>(d, g, i, t, gslot, inb, sink);
   else gs_row_step_body<false>(d, g, i, t, gslot, inb, sink);
 }

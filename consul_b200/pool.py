@@ -18,6 +18,12 @@ AGENT_STATS_DTYPE = np.dtype([(n, np.uint32) for n in AGENT_STATS_FIELDS])
 
 IMPAIR_NO_TCP = 1  # GSIM_IMPAIR_NO_TCP
 
+# gsim_domain_stats (fault domains, DESIGN.md §3.5)
+DOMAIN_MAX = (1 << 22) - 1  # GSIM_DOMAIN_MAX
+DOMAIN_STATS_DTYPE = np.dtype([(n, np.uint32) for n in ("members", "running", "paused", "impaired", "in_force",
+                                                        "alive", "suspect", "dead", "left", "awareness_max")]
+                              + [("awareness_sum", np.uint64)])
+
 PRED_RUMOR_CONVERGED = 1
 PRED_ALL_RUMORS_CONVERGED = 2
 PRED_CRASHED_ALL_DEAD = 3
@@ -343,6 +349,66 @@ class Pool:
         out = (C.c_uint64 * 4)()
         self._ck(self.lib.gsim_pause_stats(self.h, out))
         return dict(zip(("paused", "resumed_alive", "resumed_suspect", "resumed_dead"), out))
+
+    # -- fault domains (DESIGN.md §3.5 "Fault domains") -------------------------------
+    def domain_set(self, ids, domain: int):
+        """Put the listed members in fault domain `domain` (1 .. DOMAIN_MAX); 0 takes them out of any."""
+        arr = (C.c_uint32 * max(1, len(ids)))(*ids)
+        self._ck(self.lib.gsim_domain_set_many(self.h, arr, len(ids), domain))
+
+    def domain_set_range(self, first: int, count: int, per_domain: int, first_domain: int = 1):
+        """Member first + x goes to domain first_domain + x // per_domain: racks of per_domain members."""
+        self._ck(self.lib.gsim_domain_set_range(self.h, first, count, per_domain, first_domain))
+
+    def domains(self, first: int = 0, count: int | None = None) -> np.ndarray:
+        """The domain of members [first, first + count) as a uint32 array (0 = none)."""
+        if count is None:
+            count = self.stats()["n_members"] - first
+        out = np.zeros(max(count, 0), dtype=np.uint32)
+        self._ck(self.lib.gsim_domain_get(self.h, first, count, out.ctypes.data_as(C.c_void_p)))
+        return out
+
+    def domain_flap(self, domains, period_ticks: int, bad_ppm: int):
+        """Give the listed domains a flap schedule: their members' impairments are in force only during the
+        domain's bad epochs (and their own, if they have one).  period_ticks 0 clears it."""
+        arr = (C.c_uint32 * max(1, len(domains)))(*domains)
+        self._ck(self.lib.gsim_domain_flap_set(self.h, arr, len(domains), period_ticks, bad_ppm))
+
+    def domain_flap_get(self, domain: int):
+        """(period_ticks, bad_ppm) of one domain's schedule, (0, 0) without one."""
+        period, ppm = C.c_uint32(), C.c_uint32()
+        self._ck(self.lib.gsim_domain_flap_get(self.h, domain, C.byref(period), C.byref(ppm)))
+        return period.value, ppm.value
+
+    def domain_impair(self, domains, send_loss_ppm: int, recv_loss_ppm: int, delay_ticks: int = 0,
+                      flags: int = 0) -> int:
+        """impair_dir_many over every member of the listed domains; returns how many members."""
+        arr = (C.c_uint32 * max(1, len(domains)))(*domains)
+        out = C.c_uint32()
+        self._ck(self.lib.gsim_domain_impair(self.h, arr, len(domains), send_loss_ppm, recv_loss_ppm, delay_ticks,
+                                             flags, C.byref(out)))
+        return out.value
+
+    def domain_crash(self, domains) -> int:
+        """crash_many over every member of the listed domains; returns how many running members crashed."""
+        arr = (C.c_uint32 * max(1, len(domains)))(*domains)
+        out = C.c_uint32()
+        self._ck(self.lib.gsim_domain_crash(self.h, arr, len(domains), C.byref(out)))
+        return out.value
+
+    def domain_pause(self, domains, ticks: int) -> int:
+        """pause_many over every member of the listed domains; returns how many were paused."""
+        arr = (C.c_uint32 * max(1, len(domains)))(*domains)
+        out = C.c_uint32()
+        self._ck(self.lib.gsim_domain_pause(self.h, arr, len(domains), ticks, C.byref(out)))
+        return out.value
+
+    def domain_stats(self, first: int, count: int) -> np.ndarray:
+        """Per-domain counts of domains [first, first + count), read on the device, as a structured array with
+        the fields of DOMAIN_STATS_DTYPE."""
+        out = np.zeros(max(count, 0), dtype=DOMAIN_STATS_DTYPE)
+        self._ck(self.lib.gsim_domain_stats_read(self.h, first, count, out.ctypes.data_as(C.c_void_p)))
+        return out
 
     # -- time ---------------------------------------------------------------------
     def step(self, ticks: int = 1):

@@ -438,6 +438,63 @@ int gsim_pause_get(gsim_pool* p, uint32_t id, uint32_t* resume_tick);
  * refuted), resumed Dead (declared Failed, now back)}. */
 int gsim_pause_stats(gsim_pool* p, uint64_t out[4]);
 
+/* Fault domains (simulator-only fault injection: a rack switch, a hypervisor, a power feed or a zone whose
+ * members fail together; DESIGN.md §3.5 "Fault domains"):
+ *  - Every member has a domain id: 0 = none, 1 .. GSIM_DOMAIN_MAX.  The column (4 bytes per member) is
+ *    allocated by the first gsim_domain_set_* or gsim_domain_flap_set call; members added later have domain 0.
+ *  - A domain may have a flap schedule (period_ticks, bad_ppm) of the same format and range as a member's:
+ *    phase(d) = philox(seed; d, 0xFFFFFFFF, FLAP_DOMAIN = 13).y mod period, epoch = (t + phase(d)) / period,
+ *    bad(d, t) iff philox(seed; d, epoch, FLAP_DOMAIN).x < bad_ppm * 2^32 / 1e6, always for 1e6.
+ *    gsim_domain_flap_bad is this function.
+ *  - Member m's impairment (the four gsim_impair_dir_get values) is in force at tick t iff its own schedule
+ *    is absent or bad at t AND its domain is 0, has no schedule, or is bad at t.  Every "which tick" rule of
+ *    intermittent impairment applies unchanged; everything those rules leave static (accusations, fast paths,
+ *    quiet windows, gsim_health_histogram) stays static, and gsim_impair_flap_stats counts member schedules
+ *    only.
+ *  - gsim_domain_impair, _crash and _pause act on every member whose domain is listed, in one device launch
+ *    whatever the number of domains: exactly gsim_impair_dir_many, gsim_crash_many and gsim_pause_many over
+ *    those ids (a paused member crashes for good: its resume is cancelled).
+ *  - Domains and their schedules are configuration: not part of gsim_state_hash; gsim_snapshot carries the
+ *    column and the schedule table once the column exists.  Single-GPU pools only (GSIM_ERR_STATE when sharded).
+ *  - GSIM_ERR_INVALID: domain 0 or above GSIM_DOMAIN_MAX in a domain list, a range that would pass
+ *    GSIM_DOMAIN_MAX, per_domain == 0, period_ticks > 4095, bad_ppm > 1e6, and the argument rules of
+ *    gsim_impair_dir_many and gsim_pause_many.  GSIM_ERR_NOT_FOUND: an id that was never created. */
+#define GSIM_DOMAIN_MAX 4194303u /* 2^22 - 1 */
+/* Put the listed members in `domain` (0 takes them out of any domain). */
+int gsim_domain_set_many(gsim_pool* p, const uint32_t* ids, size_t n, uint32_t domain);
+/* Member first + x (x < count) goes to domain first_domain + x / per_domain: racks of per_domain members. */
+int gsim_domain_set_range(gsim_pool* p, uint32_t first, uint32_t count, uint32_t per_domain, uint32_t first_domain);
+/* out[x] = the domain of member first + x (0 on a pool that never used domains). */
+int gsim_domain_get(gsim_pool* p, uint32_t first, uint32_t count, uint32_t* out);
+/* Give the listed domains the schedule (period_ticks 1..4095, bad_ppm <= 1e6); period_ticks 0 clears it. */
+int gsim_domain_flap_set(gsim_pool* p, const uint32_t* domains, size_t n, uint32_t period_ticks, uint32_t bad_ppm);
+/* The schedule of `domain`, (0, 0) without one. */
+int gsim_domain_flap_get(gsim_pool* p, uint32_t domain, uint32_t* period_ticks, uint32_t* bad_ppm);
+/* The pure domain schedule function, like gsim_flap_bad: 1 if `domain` is in a bad epoch at `tick`, else 0; 1
+ * for period_ticks 0; GSIM_ERR_INVALID for out-of-range arguments. */
+int gsim_domain_flap_bad(uint64_t seed, uint32_t domain, uint32_t period_ticks, uint32_t bad_ppm, uint32_t tick);
+/* gsim_impair_dir_many over the members of the listed domains; *n_members = how many (may be NULL). */
+int gsim_domain_impair(gsim_pool* p, const uint32_t* domains, size_t n, uint32_t send_loss_ppm,
+                       uint32_t recv_loss_ppm, uint32_t delay_ticks, uint32_t flags, uint32_t* n_members);
+/* gsim_crash_many over the members of the listed domains; *n_crashed = running members crashed (may be NULL). */
+int gsim_domain_crash(gsim_pool* p, const uint32_t* domains, size_t n, uint32_t* n_crashed);
+/* gsim_pause_many over the members of the listed domains; *n_paused = how many were paused (may be NULL). */
+int gsim_domain_pause(gsim_pool* p, const uint32_t* domains, size_t n, uint32_t ticks, uint32_t* n_paused);
+typedef struct gsim_domain_stats {
+  uint32_t members;        /* ids in the domain whose truth is not NONE */
+  uint32_t running;        /* ... whose truth is UP */
+  uint32_t paused;         /* ... paused now (gsim_pause_get) */
+  uint32_t impaired;       /* ... with any of the four impairment values non-zero */
+  uint32_t in_force;       /* ... of those, the ones whose impairment is in force at gsim_now */
+  uint32_t alive, suspect, dead, left; /* members by the rank gsim_members reports */
+  uint32_t awareness_max;  /* over running members */
+  uint64_t awareness_sum;  /* over running members */
+} gsim_domain_stats;
+/* out[x] = the stats of domain first_domain + x, for first_domain >= 1 and first_domain + count - 1 <=
+ * GSIM_DOMAIN_MAX.  Read-only: pool state, digest, counters and schedule stay as they were; one device launch
+ * and one readback. */
+int gsim_domain_stats_read(gsim_pool* p, uint32_t first_domain, uint32_t count, gsim_domain_stats* out);
+
 /* ---- time ---------------------------------------------------------------- */
 int gsim_step(gsim_pool* p, uint32_t ticks);
 #define GSIM_PRED_RUMOR_CONVERGED 1 /* arg = slot: every UP member heard it          */
